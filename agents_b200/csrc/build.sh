@@ -1,11 +1,11 @@
 #!/usr/bin/env bash
-# Builds agents_b200/lib/libb200rl.so for sm_100a (nvcc cross-compiles without a GPU).
+# Builds agents_b200/lib/libb200rl.so for sm_90a (nvcc cross-compiles without a GPU).
 set -euo pipefail
 here="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 out="$here/../lib"
 mkdir -p "$out" "$here/obj"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-FLAGS=(-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC
+FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC --split-compile=0
        --expt-relaxed-constexpr -Xptxas -v)
 pids=()
 for f in "$here"/*.cu; do
@@ -30,5 +30,5 @@ if [[ $rc -ne 0 ]]; then
   rm -f "$out/libb200rl.so"   # never leave a stale library behind a failed build
   exit 1
 fi
-"$NVCC" -shared -gencode arch=compute_100a,code=sm_100a -o "$out/libb200rl.so" "$here"/obj/*.o -lcudart_static -ldl -lrt -lpthread
+"$NVCC" -shared -gencode arch=compute_90a,code=sm_90a -o "$out/libb200rl.so" "$here"/obj/*.o -lcudart_static -ldl -lrt -lpthread
 echo "built $out/libb200rl.so"

@@ -15,14 +15,9 @@
 // Small output grids (fc layers, filter gradients) use deterministic split-K: partial tiles
 // go to the caller's workspace and a second kernel reduces them in fixed order and applies
 // bias + activation, so results are run-to-run bit-stable.
-#include <cuda.h>
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
-
-#include <map>
-#include <mutex>
-#include <tuple>
 
 #include "common.cuh"
 
@@ -59,13 +54,10 @@ struct ARow {
   const float* p;
   int64_t ld;
   static constexpr bool kKContig = true;
-  static constexpr bool kTma2D = true;        // plain row-major [rows, K] matrix: TMA tile loads in tc2
-  static constexpr bool kLinearK = true;      // k_off(k) == k * k_stride()
   static constexpr bool kExact = false;
   __device__ __forceinline__ float at(int64_t m, int64_t k) const { return p[m * ld + k]; }
   __device__ __forceinline__ int64_t row_off(int64_t m) const { return m * ld; }
   __device__ __forceinline__ int64_t k_off(int64_t k) const { return k; }
-  __device__ __forceinline__ int64_t k_stride() const { return 1; }
   __device__ __forceinline__ bool vec4_ok() const { return (ld & 3) == 0 && ((uintptr_t)p & 15) == 0; }
   __device__ __forceinline__ float ld1(int64_t off) const { return p[off]; }
   __device__ __forceinline__ float4 ld4(int64_t off) const { return *reinterpret_cast<const float4*>(p + off); }
@@ -75,13 +67,10 @@ struct ACol {
   const float* p;
   int64_t ld;
   static constexpr bool kKContig = false;
-  static constexpr bool kTma2D = false;        // plain row-major [rows, K] matrix: TMA tile loads in tc2
-  static constexpr bool kLinearK = true;      // k_off(k) == k * k_stride()
   static constexpr bool kExact = false;
   __device__ __forceinline__ float at(int64_t m, int64_t k) const { return p[k * ld + m]; }
   __device__ __forceinline__ int64_t row_off(int64_t m) const { return m; }
   __device__ __forceinline__ int64_t k_off(int64_t k) const { return k * ld; }
-  __device__ __forceinline__ int64_t k_stride() const { return ld; }
   __device__ __forceinline__ bool vec4_ok() const { return (ld & 3) == 0 && ((uintptr_t)p & 15) == 0; }
   __device__ __forceinline__ float ld1(int64_t off) const { return p[off]; }
   __device__ __forceinline__ float4 ld4(int64_t off) const { return *reinterpret_cast<const float4*>(p + off); }
@@ -92,13 +81,10 @@ struct BRow {  // B(k, n) = p[k*ld + n]  (n contiguous)
   int64_t ld;
   static constexpr bool kNContig = true;
   static constexpr bool kKContig = false;
-  static constexpr bool kTma2D = false;        // plain row-major [rows, K] matrix: TMA tile loads in tc2
-  static constexpr bool kLinearK = true;      // k_off(k) == k * k_stride()
   static constexpr bool kExact = false;
   __device__ __forceinline__ float at(int64_t k, int64_t n) const { return p[k * ld + n]; }
   __device__ __forceinline__ int64_t row_off(int64_t n) const { return n; }
   __device__ __forceinline__ int64_t k_off(int64_t k) const { return k * ld; }
-  __device__ __forceinline__ int64_t k_stride() const { return ld; }
   __device__ __forceinline__ bool vec4_ok() const { return (ld & 3) == 0 && ((uintptr_t)p & 15) == 0; }
   __device__ __forceinline__ float ld1(int64_t off) const { return p[off]; }
   __device__ __forceinline__ float4 ld4(int64_t off) const { return *reinterpret_cast<const float4*>(p + off); }
@@ -109,13 +95,10 @@ struct BCol {  // B(k, n) = p[n*ld + k]  (k contiguous)
   int64_t ld;
   static constexpr bool kNContig = false;
   static constexpr bool kKContig = true;
-  static constexpr bool kTma2D = true;        // plain row-major [rows, K] matrix: TMA tile loads in tc2
-  static constexpr bool kLinearK = true;      // k_off(k) == k * k_stride()
   static constexpr bool kExact = false;
   __device__ __forceinline__ float at(int64_t k, int64_t n) const { return p[n * ld + k]; }
   __device__ __forceinline__ int64_t row_off(int64_t n) const { return n * ld; }
   __device__ __forceinline__ int64_t k_off(int64_t k) const { return k; }
-  __device__ __forceinline__ int64_t k_stride() const { return 1; }
   __device__ __forceinline__ bool vec4_ok() const { return (ld & 3) == 0 && ((uintptr_t)p & 15) == 0; }
   __device__ __forceinline__ float ld1(int64_t off) const { return p[off]; }
   __device__ __forceinline__ float4 ld4(int64_t off) const { return *reinterpret_cast<const float4*>(p + off); }
@@ -186,8 +169,6 @@ template <typename T>
 struct AConv {
   ConvView<T> v;
   static constexpr bool kKContig = true;
-  static constexpr bool kTma2D = false;
-  static constexpr bool kLinearK = false;
   static constexpr bool kExact = false;
   __device__ __forceinline__ float at(int64_t m, int64_t k) const {
     return v.load(v.pos_offset((uint32_t)m) + v.patch_offset((uint32_t)k));
@@ -203,8 +184,6 @@ template <typename T>
 struct AConvT {
   ConvView<T> v;
   static constexpr bool kKContig = false;
-  static constexpr bool kTma2D = false;
-  static constexpr bool kLinearK = false;
   static constexpr bool kExact = false;
   __device__ __forceinline__ float at(int64_t m, int64_t k) const {
     return v.load(v.pos_offset((uint32_t)k) + v.patch_offset((uint32_t)m));
@@ -222,8 +201,6 @@ struct AConvT {
 struct AConvU8Raw {
   ConvView<uint8_t> v;
   static constexpr bool kKContig = true;
-  static constexpr bool kTma2D = false;
-  static constexpr bool kLinearK = false;
   static constexpr bool kExact = true;
   __device__ __forceinline__ float at(int64_t m, int64_t k) const { return 0.f; }
   __device__ __forceinline__ int64_t row_off(int64_t m) const { return v.pos_offset((uint32_t)m); }
@@ -239,8 +216,6 @@ struct AConvU8Raw {
 struct AConvTU8Raw {
   ConvView<uint8_t> v;
   static constexpr bool kKContig = false;
-  static constexpr bool kTma2D = false;
-  static constexpr bool kLinearK = false;
   static constexpr bool kExact = true;
   __device__ __forceinline__ float at(int64_t m, int64_t k) const { return 0.f; }
   __device__ __forceinline__ int64_t row_off(int64_t m) const { return v.patch_offset((uint32_t)m); }
@@ -276,7 +251,6 @@ __device__ __forceinline__ float dact(float y, float g, int act) {
 
 }  // namespace b200rl
 #include "tc_gemm.cuh"
-#include "tc2_gemm.cuh"
 namespace b200rl {
 
 constexpr int BK = 16;
@@ -886,7 +860,7 @@ static int launch_gemm_cfg(const AL& a, const BL& b, const GemmArgs& g) {
   return B200RL_OK;
 }
 
-// 0 = fp32 FFMA (sgemm_kernel), 1 = tcgen05 3xTF32, 2 = tcgen05 single-pass TF32 (not 1e-5 safe)
+// 0 = fp32 FFMA (sgemm_kernel), 1 = wgmma 3xTF32, 2 = wgmma single-pass TF32 (not 1e-5 safe)
 // B200RL_FUSE_BIAS_GRAD=0 keeps the separate column-sum kernels (A/B switch for profiles/)
 static int fuse_bias_grad() {
   static int v = -1;
@@ -905,10 +879,10 @@ static int gemm_mode() {
   return g_gemm_mode;
 }
 
-template <int BN, int STAGES, int PASSES, int EPI, class AL, class BL>
+template <int BN, int PASSES, int EPI, class AL, class BL>
 static int launch_tc_cfg(const AL& a, const BL& b, const GemmArgs& g, const tc::EpiArgs& epi) {
-  using L = tc::SmemLayout<BN, STAGES, PASSES, AL::kExact>;
-  auto kernel = tc::tc_gemm_kernel<BN, STAGES, PASSES, EPI, AL, BL>;
+  using L = tc::SmemLayout<BN, PASSES, AL::kExact>;
+  auto kernel = tc::tc_gemm_kernel<BN, PASSES, EPI, AL, BL>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -922,7 +896,7 @@ static int launch_tc_cfg(const AL& a, const BL& b, const GemmArgs& g, const tc::
   const int64_t tm = (g.M + tc::kBM - 1) / tc::kBM, tn = (g.N + BN - 1) / BN;
   const int64_t tiles = tm * tn;
   int splits = 1;
-  const int64_t target = (BN <= 64 ? 2 : 1) * (int64_t)kNumSMs;  // resident CTAs on the chip
+  const int64_t target = kNumSMs;  // resident CTAs on the chip (one per SM)
   if (tiles < target && g.K >= 8 * tc::kBK && (g.ws != nullptr || EPI != tc::EPI_STORE)) {
     int64_t want = target / tiles;  // only split when a whole extra set of CTAs fits on the chip
     int64_t max_by_k = g.K / (4 * tc::kBK);
@@ -949,247 +923,16 @@ static int launch_tc_cfg(const AL& a, const BL& b, const GemmArgs& g, const tc::
 }
 
 
-// ---- second-generation (persistent, cp.async) kernel: eligibility and launch ---------------------
-// tc2 only takes operands whose every 16-byte chunk is contiguous and aligned in global memory;
-// everything else stays on tc_gemm_kernel (which has the scalar paths).
-static int g_tc2_host_flags = 0;   // bit 1: route everything to the first-generation kernel
-static int tc2_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200RL_TC2");
-    v = e ? atoi(e) : 1;
-    const char* f = getenv("B200RL_TC2_FLAGS");    // profiles/: A/B switches of tc2_gemm.cuh
-    if (f) {
-      const int flags = atoi(f);
-      g_tc2_host_flags = flags;
-      cudaMemcpyToSymbol(tc2::g_tc2_flags, &flags, sizeof(flags));
-    }
-  }
-  return v && !(g_tc2_host_flags & 2);
-}
-// Work distribution of the persistent GEMM: 0 = static striding (a few per cent faster when the
-// kernel has the GPU to itself), 1 = dynamic (global counter): CTAs whose SM is busy with a
-// collective or a kernel of another stream take fewer tiles instead of delaying the launch.  The
-// data-parallel Learner switches it on (run 17, 2 GPUs: 0.93 -> 0.946 weak-scaling efficiency
-// together with NCCL_MAX_CTAS=8).
-static int g_tile_sched = -1;
-static bool tile_scheduler_dynamic() {
-  if (g_tile_sched < 0) {
-    const char* e = getenv("B200RL_TILE_SCHED");
-    g_tile_sched = e ? (atoi(e) != 0) : 0;
-  }
-  return g_tile_sched != 0;
-}
 static bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
-static bool tc2_ok(const ARow& v, int64_t rows, int64_t K) { return (v.ld & 3) == 0 && al16(v.p) && (K & 3) == 0; }
-static bool tc2_ok(const BCol& v, int64_t rows, int64_t K) { return (v.ld & 3) == 0 && al16(v.p) && (K & 3) == 0; }
-static bool tc2_ok(const ACol& v, int64_t rows, int64_t K) { return (v.ld & 3) == 0 && al16(v.p) && (rows & 3) == 0; }
-static bool tc2_ok(const BRow& v, int64_t rows, int64_t K) { return (v.ld & 3) == 0 && al16(v.p) && (rows & 3) == 0; }
-static bool conv_f32_ok(const ConvView<float>& v) {
-  return (v.g.C & 3) == 0 && (v.g.in_img & 3) == 0 && al16(v.x);
-}
-static bool tc2_ok(const AConv<float>& v, int64_t rows, int64_t K) { return conv_f32_ok(v.v); }
-static bool tc2_ok(const AConvT<float>& v, int64_t rows, int64_t K) { return conv_f32_ok(v.v); }
-static bool conv_u8_ok(const ConvView<uint8_t>& v) {
-  const int64_t kwc = (int64_t)v.g.KW * v.g.C;
-  return (kwc & 15) == 0 && (((int64_t)v.g.stride * v.g.C) & 15) == 0 && (v.g.in_row & 15) == 0 &&
-         (v.g.in_img & 15) == 0 && al16(v.x);
-}
-static bool tc2_ok(const AConvU8Raw& v, int64_t rows, int64_t K) { return conv_u8_ok(v.v) && (K & 15) == 0; }
-static bool tc2_ok(const AConvTU8Raw& v, int64_t rows, int64_t K) { return conv_u8_ok(v.v) && (rows & 15) == 0; }
-template <class V>
-static bool tc2_ok(const V&, int64_t, int64_t) { return false; }   // AConv<uint8_t> with the exact division etc.
-
-
-// ---- TMA tensor maps for plain 2-D operands (tc2) ---------------------------------------------
-// cuTensorMapEncodeTiled is fetched through the runtime (no link against libcuda); maps are cached
-// by (base, rows, K, ld, box rows) because a training step re-launches the same GEMMs.
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-// [rows, K] fp32, row stride ld elements, tile = box_rows x 32, SWIZZLE_128B (K-major operand tile)
-static int tmap_2d(const float* base, int64_t rows, int64_t K, int64_t ld, int box_rows,
-                   CUtensorMap* out) {
-  using Key = std::tuple<const void*, int64_t, int64_t, int64_t, int>;
-  static std::map<Key, CUtensorMap> cache;
-  static std::mutex mu;
-  std::lock_guard<std::mutex> lock(mu);
-  const Key key{base, rows, K, ld, box_rows};
-  auto it = cache.find(key);
-  if (it != cache.end()) {
-    *out = it->second;
-    return B200RL_OK;
-  }
-  EncodeTiledFn fn = encode_tiled_fn();
-  if (fn == nullptr) {
-    set_error("tc2: cuTensorMapEncodeTiled is not available from this driver");
-    return B200RL_ERR_UNSUPPORTED;
-  }
-  const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  const cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(float)};
-  const cuuint32_t box[2] = {32u, (cuuint32_t)box_rows};
-  const cuuint32_t estr[2] = {1u, 1u};
-  CUtensorMap tm;
-  CUresult r = fn(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides,
-                  box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("tc2: cuTensorMapEncodeTiled failed (%d) for [%lld, %lld] ld %lld", (int)r,
-              (long long)rows, (long long)K, (long long)ld);
-    return B200RL_ERR_CUDA;
-  }
-  if (cache.size() > 4096) cache.clear();
-  cache[key] = tm;
-  *out = tm;
-  return B200RL_OK;
-}
-template <class V>
-static int tmap_for(const V&, int64_t, int64_t, int, CUtensorMap* out) {
-  memset(out, 0, sizeof(*out));
-  return B200RL_OK;
-}
-static int tmap_for(const ARow& v, int64_t rows, int64_t K, int box_rows, CUtensorMap* out) {
-  return tmap_2d(v.p, rows, K, v.ld, box_rows, out);
-}
-static int tmap_for(const BCol& v, int64_t rows, int64_t K, int box_rows, CUtensorMap* out) {
-  return tmap_2d(v.p, rows, K, v.ld, box_rows, out);
-}
-
-// operand base pointers (pair launches pass the second problem as byte offsets from the first)
-static const void* view_base(const ARow& v) { return v.p; }
-static const void* view_base(const ACol& v) { return v.p; }
-static const void* view_base(const BRow& v) { return v.p; }
-static const void* view_base(const BCol& v) { return v.p; }
-template <class T> static const void* view_base(const AConv<T>& v) { return v.v.x; }
-template <class T> static const void* view_base(const AConvT<T>& v) { return v.v.x; }
-static const void* view_base(const AConvU8Raw& v) { return v.v.x; }
-static const void* view_base(const AConvTU8Raw& v) { return v.v.x; }
-
-// second problem of a pair launch (same shapes, see tc2::PairArgs)
-template <class AL, class BL>
-struct Tc2Pair {
-  AL a;
-  BL b;
-  float* C;
-  const float* bias;
-};
-
-template <int BN, int PASSES, int EPI, class AL, class BL>
-static int launch_tc2_cfg(const AL& a, const BL& b, const GemmArgs& g, const tc::EpiArgs& epi,
-                          const Tc2Pair<AL, BL>* pair = nullptr) {
-  using L = tc2::Layout<BN, PASSES, AL::kExact>;
-  auto kernel = tc2::tc2_gemm_kernel<BN, PASSES, EPI, AL, BL>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         L::kBytes);
-    if (e != cudaSuccess) {
-      set_error("tc2_gemm: cannot set dynamic smem to %d: %s", L::kBytes, cudaGetErrorString(e));
-      return B200RL_ERR_CUDA;
-    }
-    configured = true;
-  }
-  const int64_t tm1 = (g.M + tc::kBM - 1) / tc::kBM, tn = (g.N + BN - 1) / BN;
-  const int64_t tm = pair ? 2 * tm1 : tm1;
-  const int64_t tiles = tm * tn;
-  int splits = 1;
-  const int64_t target = kNumSMs;                  // one persistent CTA per SM
-  if (tiles < target && g.K >= 8 * tc::kBK && (g.ws != nullptr || EPI != tc::EPI_STORE)) {
-    int64_t want = target / tiles;
-    int64_t max_by_k = g.K / (4 * tc::kBK);
-    int64_t max_by_ws = EPI != tc::EPI_STORE ? 65535 : g.ws_bytes / (int64_t)((pair ? 2 : 1) * g.M * g.N * sizeof(float));
-    int64_t s = want < max_by_k ? want : max_by_k;
-    if (s > max_by_ws) s = max_by_ws;
-    if (s >= 2) splits = (int)s;
-  }
-  int64_t kps = (g.K + splits - 1) / splits;
-  kps = (kps + tc::kBK - 1) / tc::kBK * tc::kBK;
-  splits = (int)((g.K + kps - 1) / kps);
-  if (splits < 1) splits = 1;
-  const int64_t total = tiles * splits;
-  B200RL_CHECK_ARG(total < (1ll << 31), "tc2_gemm: too many work items");
-  const unsigned grid = (unsigned)(total < kNumSMs ? total : kNumSMs);
-  CUtensorMap tmA, tmB, tmA2, tmB2;
-  int rc = tmap_for(a, g.M, g.K, tc::kBM, &tmA);
-  if (rc) return rc;
-  rc = tmap_for(b, g.N, g.K, BN, &tmB);
-  if (rc) return rc;
-  tmA2 = tmA;
-  tmB2 = tmB;
-  tc2::PairArgs pa{tm1, 0, 0, 0, 0};
-  if (pair) {
-    rc = tmap_for(pair->a, g.M, g.K, tc::kBM, &tmA2);
-    if (rc) return rc;
-    rc = tmap_for(pair->b, g.N, g.K, BN, &tmB2);
-    if (rc) return rc;
-    pa.a_delta = (const char*)view_base(pair->a) - (const char*)view_base(a);
-    pa.b_delta = (const char*)view_base(pair->b) - (const char*)view_base(b);
-    pa.c_delta = pair->C - g.C;
-    pa.bias_delta = (g.bias && pair->bias) ? pair->bias - g.bias : 0;
-  }
-  // epilogue-bound shapes (col2im scatter-add, short K loops) get all eight epilogue warps
-  static const int epi_env = [] { const char* e = getenv("B200RL_TC2_EPI_WARPS"); return e ? atoi(e) : 0; }();
-  const int epi_warps = (epi_env == 4 || epi_env == 8) ? epi_env
-                        : (EPI == tc::EPI_COL2IM || EPI == tc::EPI_COL2IM_MERGE || kps <= 224) ? 8 : 4;
-  // dynamic work distribution (b200rl_set_tile_scheduler) when a CTA has more than one item
-  static int sched_seq = 0;
-  int sched_slot = -1;
-  if (total > grid && tile_scheduler_dynamic()) sched_slot = (sched_seq++) & (tc2::kSchedSlots - 1);
-  B200RL_LAUNCH(kernel, grid, tc2::kThreads, L::kBytes, g.st, a, b, epi, g.C, g.bias, g.M, g.N, g.K, g.act, g.beta, splits, kps, (float*)g.ws, g.out_scale, tm, tn, epi_warps, sched_slot, pa, tmA, tmB, tmA2, tmB2);
-  B200RL_CHECK_LAUNCH("tc2_gemm");
-  if (splits > 1 && EPI == tc::EPI_STORE) {
-    const int64_t MN = g.M * g.N;
-    B200RL_LAUNCH(splitk_reduce_kernel, (unsigned)((MN + 255) / 256), 256, 0, g.st, (const float*)g.ws, g.C, g.bias, MN, g.N, splits, g.act, g.beta, g.mask);
-    B200RL_CHECK_LAUNCH("splitk_reduce");
-    if (pair) {
-      B200RL_LAUNCH(splitk_reduce_kernel, (unsigned)((MN + 255) / 256), 256, 0, g.st, (const float*)g.ws + (int64_t)splits * MN, pair->C, pair->bias, MN, g.N, splits, g.act, g.beta, g.mask);
-      B200RL_CHECK_LAUNCH("splitk_reduce");
-    }
-  }
-  return B200RL_OK;
-}
-
-// BN by N like the first-generation dispatch
-template <int PASSES, int EPI, class AL, class BL>
-static int launch_tc2(const AL& a, const BL& b, const GemmArgs& g, const tc::EpiArgs& epi,
-                      const Tc2Pair<AL, BL>* pair = nullptr) {
-  if (g.N <= 32) return launch_tc2_cfg<32, PASSES, EPI>(a, b, g, epi, pair);
-  if (g.N <= 64) return launch_tc2_cfg<64, PASSES, EPI>(a, b, g, epi, pair);
-  return launch_tc2_cfg<128, PASSES, EPI>(a, b, g, epi, pair);
-}
-template <class V> struct Tc2Capable { static constexpr bool value = true; };
-template <> struct Tc2Capable<AConv<uint8_t>> { static constexpr bool value = false; };
-template <> struct Tc2Capable<AConvT<uint8_t>> { static constexpr bool value = false; };
-template <class AL, class BL>
-static bool use_tc2(const AL& a, const BL& b, const GemmArgs& g) {
-  return tc2_enabled() && tc2_ok(a, g.M, g.K) && tc2_ok(b, g.N, g.K);
-}
 
 template <int PASSES, class AL, class BL>
 static int launch_tc(const AL& a, const BL& b, const GemmArgs& g) {
   tc::EpiArgs none{};
   none.mask = g.mask;
   B200RL_CHECK_ARG(!(g.mask.y && g.beta), "gemm: an input-gradient mask cannot be combined with accumulation");
-  if constexpr (Tc2Capable<AL>::value) {
-    if (use_tc2(a, b, g)) return launch_tc2<PASSES, tc::EPI_STORE>(a, b, g, none);
-  }
-  if (g.N <= 32) return launch_tc_cfg<32, (AL::kExact ? 4 : 2), PASSES, tc::EPI_STORE>(a, b, g, none);  // <= 96 KB -> 2 CTAs/SM
-  if (g.N <= 64) return launch_tc_cfg<64, 2, PASSES, tc::EPI_STORE>(a, b, g, none);  // 96 KB -> 2 CTAs/SM
-  return launch_tc_cfg<128, 3, PASSES, tc::EPI_STORE>(a, b, g, none);
+  if (g.N <= 32) return launch_tc_cfg<32, PASSES, tc::EPI_STORE>(a, b, g, none);
+  if (g.N <= 64) return launch_tc_cfg<64, PASSES, tc::EPI_STORE>(a, b, g, none);
+  return launch_tc_cfg<128, PASSES, tc::EPI_STORE>(a, b, g, none);
 }
 
 // Weight-gradient GEMMs (no bias / activation): in tensor-core mode the split-K partials are
@@ -1242,20 +985,14 @@ static int launch_grad_gemm(const AL& a, const BL& b, const GemmArgs& g, float* 
     none.colsum = db;
     if (db_fused) *db_fused = true;
   }
-  if constexpr (Tc2Capable<AL>::value) {
-    if (use_tc2(a, b, g)) {
-      if (mode == 2) return launch_tc2<1, tc::EPI_ATOMIC>(a, b, g, none);
-      return launch_tc2<3, tc::EPI_ATOMIC>(a, b, g, none);
-    }
-  }
   if (mode == 2) {
-    if (g.N <= 32) return launch_tc_cfg<32, (AL::kExact ? 4 : 2), 1, tc::EPI_ATOMIC>(a, b, g, none);
-    if (g.N <= 64) return launch_tc_cfg<64, 2, 1, tc::EPI_ATOMIC>(a, b, g, none);
-    return launch_tc_cfg<128, 3, 1, tc::EPI_ATOMIC>(a, b, g, none);
+    if (g.N <= 32) return launch_tc_cfg<32, 1, tc::EPI_ATOMIC>(a, b, g, none);
+    if (g.N <= 64) return launch_tc_cfg<64, 1, tc::EPI_ATOMIC>(a, b, g, none);
+    return launch_tc_cfg<128, 1, tc::EPI_ATOMIC>(a, b, g, none);
   }
-  if (g.N <= 32) return launch_tc_cfg<32, (AL::kExact ? 4 : 2), 3, tc::EPI_ATOMIC>(a, b, g, none);
-  if (g.N <= 64) return launch_tc_cfg<64, 2, 3, tc::EPI_ATOMIC>(a, b, g, none);
-  return launch_tc_cfg<128, 3, 3, tc::EPI_ATOMIC>(a, b, g, none);
+  if (g.N <= 32) return launch_tc_cfg<32, 3, tc::EPI_ATOMIC>(a, b, g, none);
+  if (g.N <= 64) return launch_tc_cfg<64, 3, tc::EPI_ATOMIC>(a, b, g, none);
+  return launch_tc_cfg<128, 3, tc::EPI_ATOMIC>(a, b, g, none);
 }
 
 
@@ -1344,71 +1081,12 @@ static int make_geom(const b200rl_conv_t* c, ConvGeom& g) {
 
 using namespace b200rl;
 
-// Forward pass of TWO layers of identical shape in one launch (DQN: the online network on
-// obs[:, 0] and the target network on obs[:, T-1]).  Falls back to two launches whenever the
-// persistent tensor-core kernel does not take the shape.
-static int pair_fwd_enabled() {
-  static const int v = [] { const char* e = getenv("B200RL_PAIR_FWD"); return e ? atoi(e) : 1; }();
-  return v;
-}
-template <class AL, class BL>
-static int launch_fwd_pair(const AL& a1, const BL& b1, const GemmArgs& g1, const AL& a2,
-                           const BL& b2, const GemmArgs& g2) {
-  const int mode = gemm_mode();
-  if constexpr (Tc2Capable<AL>::value) {
-    if (pair_fwd_enabled() && mode != 0 && g1.N >= 16 && g1.M >= 32 && g1.K >= 8 &&
-        use_tc2(a1, b1, g1) && use_tc2(a2, b2, g2) && (g1.bias == nullptr) == (g2.bias == nullptr)) {
-      tc::EpiArgs none{};
-      Tc2Pair<AL, BL> p{a2, b2, g2.C, g2.bias};
-      if (mode == 2) return launch_tc2<1, tc::EPI_STORE>(a1, b1, g1, none, &p);
-      return launch_tc2<3, tc::EPI_STORE>(a1, b1, g1, none, &p);
-    }
-  }
-  int rc = launch_gemm(a1, b1, g1);
-  if (rc) return rc;
-  return launch_gemm(a2, b2, g2);
-}
-
-
 extern "C" {
 
 int b200rl_tc_debug_buffer(long long* dev_buf) {
   cudaError_t e = cudaMemcpyToSymbol(tc::g_tc_dbg, &dev_buf, sizeof(dev_buf));
   if (e != cudaSuccess) {
     set_error("tc_debug_buffer: %s", cudaGetErrorString(e));
-    return B200RL_ERR_CUDA;
-  }
-  return B200RL_OK;
-}
-
-int b200rl_tc_debug_variant(int v) {
-  cudaError_t e = cudaMemcpyToSymbol(tc::g_tc_variant, &v, sizeof(v));
-  if (e != cudaSuccess) {
-    set_error("tc_debug_variant: %s", cudaGetErrorString(e));
-    return B200RL_ERR_CUDA;
-  }
-  return B200RL_OK;
-}
-
-int b200rl_tc2_trace_buffer(long long* dev_buf) {
-  cudaError_t e = cudaMemcpyToSymbol(tc2::g_tc2_trace, &dev_buf, sizeof(dev_buf));
-  if (e != cudaSuccess) {
-    set_error("tc2_trace_buffer: %s", cudaGetErrorString(e));
-    return B200RL_ERR_CUDA;
-  }
-  return B200RL_OK;
-}
-
-int b200rl_set_tile_scheduler(int dynamic) {
-  g_tile_sched = dynamic ? 1 : 0;
-  return B200RL_OK;
-}
-
-int b200rl_set_tc2_flags(int flags) {
-  g_tc2_host_flags = flags;
-  cudaError_t e = cudaMemcpyToSymbol(tc2::g_tc2_flags, &flags, sizeof(flags));
-  if (e != cudaSuccess) {
-    set_error("set_tc2_flags: %s", cudaGetErrorString(e));
     return B200RL_ERR_CUDA;
   }
   return B200RL_OK;
@@ -1452,8 +1130,8 @@ static int thin_dw_launch(const float* X, int64_t ldx, const float* dZ, float* d
 }
 
 int b200rl_set_gemm_mode(int mode) {
-  B200RL_CHECK_ARG(mode >= 0 && mode <= 2, "gemm mode must be 0 (fp32 FFMA), 1 (tcgen05 3xTF32) "
-                                           "or 2 (tcgen05 1xTF32)");
+  B200RL_CHECK_ARG(mode >= 0 && mode <= 2, "gemm mode must be 0 (fp32 FFMA), 1 (wgmma 3xTF32) "
+                                           "or 2 (wgmma 1xTF32)");
   g_gemm_mode = mode;
   return B200RL_OK;
 }
@@ -1485,7 +1163,9 @@ int b200rl_dense_fwd_pair(const float* X1, const float* X2, int64_t ldx, const f
   }
   GemmArgs g1{Y1, bias1, M, N, K, act, 0, workspace, ws_bytes, (cudaStream_t)stream};
   GemmArgs g2{Y2, bias2, M, N, K, act, 0, workspace, ws_bytes, (cudaStream_t)stream};
-  return launch_fwd_pair(ARow{X1, ldx ? ldx : K}, BRow{W1, N}, g1, ARow{X2, ldx ? ldx : K}, BRow{W2, N}, g2);
+  int rc = launch_gemm(ARow{X1, ldx ? ldx : K}, BRow{W1, N}, g1);
+  if (rc) return rc;
+  return launch_gemm(ARow{X2, ldx ? ldx : K}, BRow{W2, N}, g2);
 }
 
 int b200rl_dense_bwd(const float* X, int64_t ldx, const float* W, const float* dY, float* dX,
@@ -1586,12 +1266,6 @@ int b200rl_conv2d_fwd_pair(const void* X1, const void* X2, int x_is_u8, float x_
       AConvU8Raw a1{ConvView<uint8_t>{(const uint8_t*)X1, cg, x_scale}};
       AConvU8Raw a2{ConvView<uint8_t>{(const uint8_t*)X2, cg, x_scale}};
       const BRow b1{Wt1, c->F}, b2{Wt2, c->F};
-      if (pair_fwd_enabled() && use_tc2(a1, b1, g1) && use_tc2(a2, b2, g2) &&
-          (bias1 == nullptr) == (bias2 == nullptr)) {
-        tc::EpiArgs none{};
-        Tc2Pair<AConvU8Raw, BRow> p{a2, b2, Y2, bias2};
-        return launch_tc2<3, tc::EPI_STORE>(a1, b1, g1, none, &p);
-      }
       rc = launch_tc<3>(a1, b1, g1);
       if (rc) return rc;
       return launch_tc<3>(a2, b2, g2);
@@ -1602,7 +1276,9 @@ int b200rl_conv2d_fwd_pair(const void* X1, const void* X2, int x_is_u8, float x_
   }
   AConv<float> a1{ConvView<float>{(const float*)X1, cg, 1.f}};
   AConv<float> a2{ConvView<float>{(const float*)X2, cg, 1.f}};
-  return launch_fwd_pair(a1, BRow{Wt1, c->F}, g1, a2, BRow{Wt2, c->F}, g2);
+  rc = launch_gemm(a1, BRow{Wt1, c->F}, g1);
+  if (rc) return rc;
+  return launch_gemm(a2, BRow{Wt2, c->F}, g2);
 }
 
 int b200rl_conv2d_bwd(const void* X, int x_is_u8, float x_scale, const float* Wt,
@@ -1641,7 +1317,7 @@ int b200rl_conv2d_bwd(const void* X, int x_is_u8, float x_scale, const float* Wt
     if (rc) return rc;
   }
   if (dX && gemm_mode() != 0 && (c->C & 3) == 0 && K >= 16 && M >= 32 && F >= 8) {
-    // tcgen05 path: dY @ W^T with the col2im scatter-add fused into the epilogue
+    // tensor-core path: dY @ W^T with the col2im scatter-add fused into the epilogue
     const int64_t total = (int64_t)c->N * c->H * c->W * c->C;
     cudaError_t e = cudaMemsetAsync(dX, 0, (size_t)total * sizeof(float), st);
     if (e != cudaSuccess) {
@@ -1653,19 +1329,8 @@ int b200rl_conv2d_bwd(const void* X, int x_is_u8, float x_scale, const float* Wt
     epi.mask = mask;
     const ARow da{dY, F};
     const BCol db_{Wt, F};
-    // neighbour pre-sum of the col2im epilogue (tc2_gemm.cuh): the partner column group sits
-    // stride * C = 64 columns away, i.e. in the other half of the same 128-column tile (the Mnih
-    // conv2 (k4 s2 C32) and conv3 (k3 s1 C64) input gradients); B200RL_COL2IM_MERGE=0 turns it off
-    static const int merge_env = [] { const char* e = getenv("B200RL_COL2IM_MERGE"); return e ? atoi(e) : 1; }();
-    if (merge_env && (int64_t)c->stride * c->C == 64 && (c->C & 15) == 0 && cg.OW > 1) epi.merge_cols = 64;
-    if (use_tc2(da, db_, g)) {
-      if (epi.merge_cols) {
-        if (gemm_mode() == 2) rc = launch_tc2_cfg<128, 1, tc::EPI_COL2IM_MERGE>(da, db_, g, epi);
-        else rc = launch_tc2_cfg<128, 3, tc::EPI_COL2IM_MERGE>(da, db_, g, epi);
-      } else if (gemm_mode() == 2) rc = launch_tc2_cfg<128, 1, tc::EPI_COL2IM>(da, db_, g, epi);
-      else rc = launch_tc2_cfg<128, 3, tc::EPI_COL2IM>(da, db_, g, epi);
-    } else if (gemm_mode() == 2) rc = launch_tc_cfg<128, 3, 1, tc::EPI_COL2IM>(da, db_, g, epi);
-    else rc = launch_tc_cfg<128, 3, 3, tc::EPI_COL2IM>(da, db_, g, epi);
+    if (gemm_mode() == 2) rc = launch_tc_cfg<128, 1, tc::EPI_COL2IM>(da, db_, g, epi);
+    else rc = launch_tc_cfg<128, 3, tc::EPI_COL2IM>(da, db_, g, epi);
     if (rc) return rc;
   } else if (dX) {  // dcol[M,K] = dY @ W^T, then gather-form col2im
     const int64_t need = M * K * (int64_t)sizeof(float);

@@ -19,7 +19,7 @@ namespace b200rl {
 
 constexpr float kLog2Pi = 1.8378770664093453f;
 constexpr int kStepLastP = 2;
-constexpr int kRedBlocks = 296;  // 2 x 148 SMs
+constexpr int kRedBlocks = 2 * kNumSMs;
 
 struct PpoArgs {
   const float* loc; const float* scale; int64_t ld_ls;      // current policy Normal(loc, scale)

@@ -1,27 +1,26 @@
-// Tensor-core GEMM for the Q / actor / critic networks: tcgen05.mma (kind::tf32) with TMEM
-// accumulators, fp32-grade accuracy through the 3xTF32 split.
+// Tensor-core GEMM for the Q / actor / critic networks: Hopper warpgroup MMA (wgmma, tf32 inputs,
+// fp32 register accumulators), fp32-grade accuracy through the 3xTF32 split.
 //
 //   C[M,N] (+)= act(A[M,K] @ B[K,N] + bias)      A, B given as operand views (see nn.cu)
 //
 // Why 3xTF32: north_star parity is 1e-5 relative on the loss; one TF32 pass keeps ~11 mantissa
 // bits (1e-3).  Each fp32 operand x is split in registers into hi = x with the low 13 mantissa
 // bits cleared and lo = x - hi (exact); the tensor core accumulates lo_a*hi_b + hi_a*lo_b +
-// hi_a*hi_b into the same fp32 TMEM accumulator (the dropped lo*lo term is 2^-22 relative).
+// hi_a*hi_b into the same fp32 accumulator (the dropped lo*lo term is 2^-22 relative).
 //
-// Structure (one CTA = one 128 x BN output tile, cta_group::1, 9 warps):
-//   warps 0-7  producers: gather a (128 x 32) A tile and a (BN x 32) B^T tile of fp32 through
-//              the operand views (implicit im2col, u8->f32 cast, transposes all happen here),
-//              split hi/lo, store them K-major into 128B-swizzled shared memory (the layout a
-//              TMA SWIZZLE_128B load would produce), fence.proxy.async, arrive on full[s];
-//              after the main loop the same 4 warps are the epilogue (tcgen05.ld 32x32b:
-//              warp w owns TMEM lanes 32w..32w+31), apply bias/activation, store C or the
-//              split-K partial.
-//   warp 8     allocates TMEM (BN fp32 columns), lane 0 issues tcgen05.mma for every K step
-//              (K = 8 per instruction for tf32; 4 steps x 3 passes per 32-wide K block),
-//              releases stages with tcgen05.commit -> empty[s], signals the epilogue with a
-//              final commit.
-// Descriptors follow cute/arch/mma_sm100_desc.hpp (SmemDescriptor: K-major SWIZZLE_128B,
-// SBO = 1024 B, version 1; InstrDescriptor: F32 accumulate, TF32 x TF32, M = 128, N = BN).
+// Structure (one CTA = one 128 x BN output tile, 256 threads = two warpgroups):
+//   every thread gathers its share of a (128 x 32) A tile and a (BN x 32) B^T tile through the
+//   operand views (implicit im2col, u8->f32 cast and transposes happen here; the global loads of
+//   K block i+1 are in flight while block i is split and stored), splits hi/lo and stores them
+//   K-major into 128B-swizzled shared memory, the layout wgmma reads (tf32 operands must be
+//   K-major, so MN-contiguous views are transposed on the way in);
+//   after one CTA barrier per K block, warpgroup w issues wgmma.m64nBNk8 for rows 64w..64w+63
+//   (4 K steps x up to 3 passes per 32-wide K block) and keeps one group in flight while the
+//   next block is stored: three stages make one barrier per K block sufficient (the stage
+//   written in block i was last read by the MMAs of block i-3, which every warpgroup retired
+//   before the barrier of block i-1).
+//   The epilogue parks the accumulators in the idle stage buffers and drains them row-per-thread:
+//   bias / activation / act' mask / split-K partials, the fused col2im scatter-add, or red.add.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -31,19 +30,11 @@ namespace tc {
 
 constexpr int kBM = 128;
 constexpr int kBK = 32;                    // fp32 elements = 128 bytes = one swizzle row
-constexpr int kProducerThreads = 256;
-constexpr int kThreads = 288;
+constexpr int kThreads = 256;
+constexpr int kStages = 3;
 
 // optional phase stamps (b200rl_tc_debug_buffer): [block][8] nanosecond timers
 __device__ long long* g_tc_dbg = nullptr;
-// Pipeline ablations (profiles/tc_ablate.py) are compiled in only with -DB200RL_TC_ABLATE; the
-// production library ignores b200rl_tc_debug_variant.
-__device__ int g_tc_variant = 0;
-#ifdef B200RL_TC_ABLATE
-#define TC_ABL(v) (v)
-#else
-#define TC_ABL(v) 0
-#endif
 __device__ __forceinline__ long long gtimer() {
   long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -59,93 +50,79 @@ __device__ __forceinline__ void stamp(int slot) {
 __device__ __forceinline__ uint32_t smem_addr(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// Non-blocking test_wait poll (the blocking try_wait form faulted in this kernel on the r1 pool,
-// see profiles/README.md; polling by one lane per warp measured the same as polling by all).
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 
-// K-major, SWIZZLE_128B, 8-row groups 1024 B apart (cute SmemDescriptor, version 1).
+// Shared-memory matrix descriptor (sm_90 GMMA): K-major, SWIZZLE_128B, 8-row groups 1024 B apart.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);          // start address
   d |= (uint64_t)1 << 16;                          // leading byte offset (unused for SW128 K-major)
   d |= (uint64_t)(1024 >> 4) << 32;                // stride byte offset
-  d |= (uint64_t)1 << 46;                          // version = 1 (sm_100)
-  d |= (uint64_t)2 << 61;                          // layout type SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                          // layout type 1 = SWIZZLE_128B
   return d;
-}
-// MN-major tf32 operands: SWIZZLE_128B_BASE32B is the only layout the tensor core accepts for
-// 32-bit MN-major data (cutlass sm100_common.inl: "for mn-major tf32 operands, SW128_32B is the
-// only available smem layout"; cute Layout_MN_SW128_32B_Atom = Swizzle<2,5,2> o (1024 bit, 4) :
-// (1, 1024 bit)).  A k-row holds 32 consecutive M/N elements (128 B); 4 k-rows form a 512 B atom
-// in which the 32-byte blocks of a row are XORed with the row index; LBO = distance between
-// 32-element M/N groups, SBO = distance between 4-row k atoms (one K=8 MMA spans two atoms).
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)(512 >> 4) << 16;                 // LBO: next 32-row M/N group (adjacent atom)
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;  // SBO: next 4-row k atom = (ROWS/32) atoms
-  d |= (uint64_t)1 << 46;                          // version = 1 (sm_100)
-  d |= (uint64_t)1 << 61;                          // layout type 1 = SWIZZLE_128B_BASE32B
-  return d;
-}
-__host__ __device__ constexpr uint32_t make_idesc(int bn, bool a_mn, bool b_mn) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-         ((uint32_t)(bn >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);
-}
-// byte offset of the 16-byte chunk holding rows 4*cm..4*cm+3 at reduction index k (0..31) in an
-// MN-major tile: 512 B atoms (32 rows x 4 k) tiled M/N-fastest, rows 128 B apart;
-// inside a row the 32-byte block index is XORed with (k & 3).
-template <int ROWS>
-__device__ __forceinline__ uint32_t mn128(uint32_t cm, uint32_t k) {
-  // atoms are tiled M/N-fastest (the arrangement cute's tile_to_shape produces)
-  const uint32_t c = cm & 7u, kin = k & 3u;
-  const uint32_t blk = (((c >> 1) ^ kin) << 1) | (c & 1u);   // 32-byte block XOR k, 16 B half kept
-  return ((k >> 2) * (ROWS / 32) + (cm >> 3)) * 512u + kin * 128u + (blk << 4);
 }
 
-// byte offset of 16-byte chunk j (0..7) of row r inside a K-major [rows x 128 B] SWIZZLE_128B tile
+// D[64 x N] += A[64 x 8] * B[8 x N], both operands from shared memory (descriptors above).
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t a, uint64_t b);
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(1));
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+
+// byte offset of the 16-byte chunk j (0..7) of row r inside a K-major [rows x 128 B] SWIZZLE_128B tile
 __device__ __forceinline__ uint32_t sw128(uint32_t r, uint32_t j) {
   return (r >> 3) * 1024u + (r & 7u) * 128u + ((j ^ (r & 7u)) << 4);
+}
+
+__device__ __forceinline__ float tf32_hi(float x) {
+  return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
 }
 
 template <bool WITH_LO>
 __device__ __forceinline__ void split_store(unsigned char* hi_tile, unsigned char* lo_tile,
                                             uint32_t off, float4 v) {
   float4 h;
-  h.x = __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
-  h.y = __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-  h.z = __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
-  h.w = __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
+  h.x = tf32_hi(v.x);
+  h.y = tf32_hi(v.y);
+  h.z = tf32_hi(v.z);
+  h.w = tf32_hi(v.w);
   // explicit st.shared: the tile pointers come from integer alignment arithmetic, which makes
   // the compiler fall back to generic ST.E otherwise
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(smem_addr(hi_tile) + off),
@@ -157,17 +134,27 @@ __device__ __forceinline__ void split_store(unsigned char* hi_tile, unsigned cha
                  : "memory");
   }
 }
+template <bool WITH_LO>
+__device__ __forceinline__ void split_store1(unsigned char* hi_tile, unsigned char* lo_tile,
+                                             uint32_t off, float v) {
+  const float h = tf32_hi(v);
+  asm volatile("st.shared.f32 [%0], %1;" ::"r"(smem_addr(hi_tile) + off), "f"(h) : "memory");
+  if (WITH_LO)
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(smem_addr(lo_tile) + off), "f"(v - h) : "memory");
+}
 
 // A_EXACT: the A view yields values that are exactly representable in TF32 (raw uint8 pixels), so
 // A needs no "lo" plane and the product needs only 2 passes (a*b_lo + a*b_hi).
-template <int BN, int STAGES, int PASSES, bool A_EXACT = false>
+template <int BN, int PASSES, bool A_EXACT = false>
 struct SmemLayout {
   static constexpr int kATile = kBM * 128;
   static constexpr int kBTile = BN * 128;
   static constexpr int kNumA = (PASSES == 3 && !A_EXACT) ? 2 : 1;   // A planes
   static constexpr int kNumB = PASSES == 3 ? 2 : 1;                 // B planes
   static constexpr int kStage = kNumA * kATile + kNumB * kBTile;
-  static constexpr int kBytes = STAGES * kStage + 1024 /*alignment slack*/ + 256 /*barriers*/ + BN * 4 /*bias*/;
+  static constexpr int kPitch = BN + 4;                             // epilogue staging row (floats)
+  static_assert(kBM * kPitch * 4 <= kStages * kStage, "epilogue staging tile must fit");
+  static constexpr int kBytes = kStages * kStage + 1024 /*alignment slack*/ + BN * 4 /*bias*/;
 };
 
 // One chunk = 4 consecutive k of one row.  roff = view.row_off(row); koff[i] = view.k_off(k+i).
@@ -176,7 +163,7 @@ __device__ __forceinline__ float4 load_chunk(const V& v, int64_t roff, bool row_
                                              int64_t ke, const int64_t (&koff)[4], bool full_vec) {
   float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
   if (!row_ok || k >= ke) return r;
-  if (V::kKContig && full_vec) return v.ld4(roff + koff[0]);
+  if (full_vec) return v.ld4(roff + koff[0]);
   r.x = v.ld1(roff + koff[0]);
   if (k + 1 < ke) r.y = v.ld1(roff + koff[1]);
   if (k + 2 < ke) r.z = v.ld1(roff + koff[2]);
@@ -185,64 +172,59 @@ __device__ __forceinline__ float4 load_chunk(const V& v, int64_t roff, bool row_
 }
 
 // A [ROWS x 32] fp32 operand tile is moved in two steps so that the global loads of K block i+1
-// are in flight while block i is split and stored: gather_tile (global -> registers) and
-// scatter_tile (registers -> hi/lo planes in 128B-swizzled shared memory).
+// are in flight while block i is split and stored: gather (global -> registers) and scatter
+// (registers -> hi/lo planes in 128B-swizzled shared memory).
 // K-contiguous views: thread = (row group tid>>3, chunk tid&7), 8 lanes read 128 contiguous
-// bytes of a row; row_offs[i] belongs to row (tid>>3) + 32 i.  Other views: thread = (row
-// tid % ROWS, chunks tid/ROWS + TPR i): consecutive lanes read consecutive rows (coalesced) and
-// the XOR swizzle makes the 16-byte stores of 8 consecutive rows hit 8 distinct bank groups.
+// bytes of a row; row_offs[i] belongs to row (tid>>3) + 32 i.
 template <int ROWS, class V>
 __device__ __forceinline__ void gather_tile(const V& v, const int64_t* row_offs,
                                             uint32_t row_ok_mask, int64_t k0, int64_t ke, bool vec,
-                                            int tid, float4 (&val)[ROWS * 8 / kProducerThreads]) {
-  constexpr int NV = ROWS * 8 / kProducerThreads;
-  if (V::kKContig) {
-    const int j = tid & 7;
-    const int64_t k = k0 + j * 4;
-    const bool full_vec = vec && (k + 3 < ke);
-    int64_t koff[4];
-    koff[0] = k < ke ? v.k_off(k) : 0;
+                                            int tid, float4 (&val)[ROWS * 8 / kThreads]) {
+  constexpr int NV = ROWS * 8 / kThreads;
+  const int j = tid & 7;
+  const int64_t k = k0 + j * 4;
+  const bool full_vec = vec && (k + 3 < ke);
+  int64_t koff[4];
+  koff[0] = k < ke ? v.k_off(k) : 0;
 #pragma unroll
-    for (int i = 1; i < 4; ++i) koff[i] = (!full_vec && k + i < ke) ? v.k_off(k + i) : 0;
+  for (int i = 1; i < 4; ++i) koff[i] = (!full_vec && k + i < ke) ? v.k_off(k + i) : 0;
 #pragma unroll
-    for (int i = 0; i < NV; ++i)
-      val[i] = load_chunk(v, row_offs[i], (row_ok_mask >> i) & 1u, k, ke, koff, full_vec);
-  } else {
-    constexpr int TPR = kProducerThreads / ROWS;  // threads per row
-    const int jb = tid / ROWS;
-    // k_off depends on k only (for the conv filter-gradient view it is a full (n, oy, ox) decode):
-    // lane l computes it for k0 + l once and the 4 offsets of each chunk are fetched by shuffle.
-    const int lane = tid & 31;
-    const int64_t my_koff = (k0 + lane < ke) ? v.k_off(k0 + lane) : 0;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      const int j = jb + TPR * i;
-      const int64_t k = k0 + j * 4;
-      int64_t koff[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) koff[q] = __shfl_sync(0xffffffffu, my_koff, j * 4 + q);
-      val[i] = load_chunk(v, row_offs[0], row_ok_mask & 1u, k, ke, koff, false);
-    }
-  }
+  for (int i = 0; i < NV; ++i)
+    val[i] = load_chunk(v, row_offs[i], (row_ok_mask >> i) & 1u, k, ke, koff, full_vec);
 }
 
-// MN-major tiles (views whose M/N index is contiguous in memory): thread = (row chunk cm =
-// tid % (ROWS/4), k = tid / (ROWS/4) + KSTEP i).  A warp reads up to 512 contiguous bytes of one
-// k-row with 16-byte vectors; no transposition is needed because the MMA descriptor is MN-major.
+template <int ROWS, bool WITH_LO>
+__device__ __forceinline__ void scatter_tile(unsigned char* hi, unsigned char* lo, int tid,
+                                             const float4 (&val)[ROWS * 8 / kThreads]) {
+  constexpr int NV = ROWS * 8 / kThreads;
+#pragma unroll
+  for (int i = 0; i < NV; ++i)
+    split_store<WITH_LO>(hi, lo, sw128((uint32_t)((tid >> 3) + 32 * i), (uint32_t)(tid & 7)), val[i]);
+}
+
+// MN-contiguous views (the M/N index is contiguous in memory): chunk c = tid + 256 i holds rows
+// 4 cm .. 4 cm + 3 at reduction index k, with k & 7 = c & 7, cm = (c >> 3) % CPR and
+// k >> 3 = (c >> 3) / CPR.  A warp reads 8 k-rows x 64 contiguous bytes; the transposing scalar
+// stores of a warp then spread over 16 banks (2-way conflicts instead of 16-way for a
+// row-per-lane map).  cm does not depend on i, so every chunk of a thread covers the same 4
+// columns (the fused bias gradient relies on it).
+template <int ROWS>
+struct MnMap {
+  static constexpr int CPR = ROWS / 4;
+  __device__ static __forceinline__ int cm(int c) { return (c >> 3) % CPR; }
+  __device__ static __forceinline__ int kk(int c) { return (c & 7) | (((c >> 3) / CPR) << 3); }
+};
 template <int ROWS, class V>
 __device__ __forceinline__ void gather_tile_mn(const V& v, int64_t row0, int64_t row_limit,
                                                int64_t k0, int64_t ke, bool vec, int tid,
-                                               float4 (&val)[ROWS * 8 / kProducerThreads]) {
-  constexpr int NV = ROWS * 8 / kProducerThreads;
-  constexpr int CPR = ROWS / 4;                      // chunks per k-row
-  constexpr int KSTEP = kProducerThreads / CPR;      // k-rows covered per pass
-  const int cm = tid % CPR;
-  const int64_t r = row0 + 4 * cm;
+                                               float4 (&val)[ROWS * 8 / kThreads]) {
+  constexpr int NV = ROWS * 8 / kThreads;
+  const int64_t r = row0 + 4 * MnMap<ROWS>::cm(tid);
   const int64_t roff = r < row_limit ? v.row_off(r) : 0;
   const bool row_full = r + 3 < row_limit;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
-    const int64_t k = k0 + tid / CPR + KSTEP * i;
+    const int64_t k = k0 + MnMap<ROWS>::kk(tid + kThreads * i);
     float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
     if (k < ke && r < row_limit) {
       const int64_t off = roff + v.k_off(k);
@@ -258,31 +240,19 @@ __device__ __forceinline__ void gather_tile_mn(const V& v, int64_t row0, int64_t
     val[i] = x;
   }
 }
-
 template <int ROWS, bool WITH_LO>
 __device__ __forceinline__ void scatter_tile_mn(unsigned char* hi, unsigned char* lo, int tid,
-                                                const float4 (&val)[ROWS * 8 / kProducerThreads]) {
-  constexpr int NV = ROWS * 8 / kProducerThreads;
-  constexpr int CPR = ROWS / 4;
-  constexpr int KSTEP = kProducerThreads / CPR;
+                                                const float4 (&val)[ROWS * 8 / kThreads]) {
+  constexpr int NV = ROWS * 8 / kThreads;
+  const uint32_t r = 4u * (uint32_t)MnMap<ROWS>::cm(tid);
 #pragma unroll
-  for (int i = 0; i < NV; ++i)
-    split_store<WITH_LO>(hi, lo, mn128<ROWS>((uint32_t)(tid % CPR), (uint32_t)(tid / CPR + KSTEP * i)), val[i]);
-}
-
-template <int ROWS, bool WITH_LO, bool KCONTIG>
-__device__ __forceinline__ void scatter_tile(unsigned char* hi, unsigned char* lo, int tid,
-                                             const float4 (&val)[ROWS * 8 / kProducerThreads]) {
-  constexpr int NV = ROWS * 8 / kProducerThreads;
-  if (KCONTIG) {
-#pragma unroll
-    for (int i = 0; i < NV; ++i)
-      split_store<WITH_LO>(hi, lo, sw128((uint32_t)((tid >> 3) + 32 * i), (uint32_t)(tid & 7)), val[i]);
-  } else {
-    constexpr int TPR = kProducerThreads / ROWS;
-#pragma unroll
-    for (int i = 0; i < NV; ++i)
-      split_store<WITH_LO>(hi, lo, sw128((uint32_t)(tid % ROWS), (uint32_t)(tid / ROWS + TPR * i)), val[i]);
+  for (int i = 0; i < NV; ++i) {
+    const uint32_t k = (uint32_t)MnMap<ROWS>::kk(tid + kThreads * i);
+    const uint32_t j = k >> 2, e = (k & 3u) * 4u;
+    split_store1<WITH_LO>(hi, lo, sw128(r + 0, j) + e, val[i].x);
+    split_store1<WITH_LO>(hi, lo, sw128(r + 1, j) + e, val[i].y);
+    split_store1<WITH_LO>(hi, lo, sw128(r + 2, j) + e, val[i].z);
+    split_store1<WITH_LO>(hi, lo, sw128(r + 3, j) + e, val[i].w);
   }
 }
 
@@ -295,42 +265,32 @@ __device__ __forceinline__ void scatter_tile(unsigned char* hi, unsigned char* l
 constexpr int EPI_STORE = 0;
 constexpr int EPI_COL2IM = 1;
 constexpr int EPI_ATOMIC = 2;  // C += acc with red.global.add (split-K without a reduce pass; C pre-zeroed)
-// tc2 kernel only: EPI_COL2IM with the neighbour pre-sum of EpiArgs::merge_cols (its own
-// instantiation, so that neither variant pays for the other's registers)
-constexpr int EPI_COL2IM_MERGE = 3;
 struct EpiArgs {
   ConvGeom g;
   float* dx;
   ActMask mask;     // EPI_STORE / EPI_COL2IM: multiply the input gradient by act'(mask.y)
   float* colsum;    // EPI_ATOMIC with an MN-major B view: column sums of B (bias gradient) += here
-  // EPI_COL2IM (tc2 kernel only): columns c and c + merge_cols (= stride * C) of NEIGHBOURING output
-  // positions (ox + 1, ox) address the same input element; when != 0 the epilogue adds them with a
-  // lane shuffle before the red.global.add (see tc2_gemm.cuh).  0: every column group is scattered.
-  int merge_cols;
 };
 
 // AL / BL are the fp32 operand views of nn.cu (row index = m for A, n for B).
-template <int BN, int STAGES, int PASSES, int EPI, class AL, class BL>
-__global__ void __launch_bounds__(kThreads, (BN <= 64 ? 2 : 1)) tc_gemm_kernel(const AL a, const BL b,
-                                                           const EpiArgs epi,
-                                                           float* __restrict__ C,
-                                                           const float* __restrict__ bias,
-                                                           int64_t M, int64_t N, int64_t K, int act,
-                                                           int beta, int splits,
-                                                           int64_t k_per_split,
-                                                           float* __restrict__ ws,
-                                                           float out_scale) {
-  using L = SmemLayout<BN, STAGES, PASSES, AL::kExact>;
+template <int BN, int PASSES, int EPI, class AL, class BL>
+__global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const BL b,
+                                                              const EpiArgs epi,
+                                                              float* __restrict__ C,
+                                                              const float* __restrict__ bias,
+                                                              int64_t M, int64_t N, int64_t K,
+                                                              int act, int beta, int splits,
+                                                              int64_t k_per_split,
+                                                              float* __restrict__ ws,
+                                                              float out_scale) {
+  using L = SmemLayout<BN, PASSES, AL::kExact>;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  unsigned char* bars = smem + STAGES * L::kStage;
-  unsigned long long* full = reinterpret_cast<unsigned long long*>(bars);
-  unsigned long long* empty = full + STAGES;
-  unsigned long long* accum = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum + 1);
+  float* sbias = reinterpret_cast<float*>(smem + kStages * L::kStage);   // bias slice / column sums
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = tid >> 7;                                  // warpgroup: tile rows 64 wg ..
   const int64_t m0 = (int64_t)blockIdx.y * kBM, n0 = (int64_t)blockIdx.x * BN;
   const int split = blockIdx.z;
   const int64_t kb = (int64_t)split * k_per_split;
@@ -339,319 +299,261 @@ __global__ void __launch_bounds__(kThreads, (BN <= 64 ? 2 : 1)) tc_gemm_kernel(c
 
   pdl_launch_dependents();   // the next kernel of the stream may be scheduled from here on
   if (tid == 0) stamp(0);
-  float* sbias = reinterpret_cast<float*>(bars + 256);   // bias slice (EPI_STORE) / column sums
   if (EPI == EPI_ATOMIC && tid < BN) sbias[tid] = 0.f;
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(smem_addr(&full[s]), kProducerThreads / 32);  // one arrive per producer warp
-      mbar_init(smem_addr(&empty[s]), 1);   // tcgen05.commit
-    }
-    mbar_init(smem_addr(accum), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 8) {
-    constexpr int kCols = BN < 32 ? 32 : BN;
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_addr(tmem_slot)),
-                 "n"(kCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
   // everything above touched no global memory; from here on the producing kernels must be done
   pdl_wait();
   if (tid == 0) stamp(1);
 
-  if (warp < 8) {
-    // ===================== producers =====================
-    constexpr bool kLo = PASSES == 3;
-    constexpr bool kLoA = PASSES == 3 && !AL::kExact;
-    constexpr int NRA = AL::kKContig ? kBM * 8 / kProducerThreads : 1;
-    constexpr int NRB = BL::kKContig ? BN * 8 / kProducerThreads : 1;
-    static_assert(BN * 8 >= kProducerThreads, "BN must be >= 32");
-    int64_t a_off[NRA], b_off[NRB];
-    uint32_t a_ok = 0, b_ok = 0;
+  constexpr bool kLo = PASSES == 3;
+  constexpr bool kLoA = PASSES == 3 && !AL::kExact;
+  constexpr int NRA = AL::kKContig ? kBM * 8 / kThreads : 1;
+  constexpr int NRB = BL::kKContig ? BN * 8 / kThreads : 1;
+  static_assert(BN * 8 >= kThreads, "BN must be >= 32");
+  int64_t a_off[NRA], b_off[NRB];
+  uint32_t a_ok = 0, b_ok = 0;
+  if (AL::kKContig) {
 #pragma unroll
     for (int i = 0; i < NRA; ++i) {  // hoisted row offsets (implicit-im2col index math runs once)
-      const int r = AL::kKContig ? (tid >> 3) + 32 * i : tid % kBM;
+      const int r = (tid >> 3) + 32 * i;
       const bool ok = m0 + r < M;
       a_off[i] = ok ? a.row_off(m0 + r) : 0;
       a_ok |= (ok ? 1u : 0u) << i;
     }
+  }
+  if (BL::kKContig) {
 #pragma unroll
     for (int i = 0; i < NRB; ++i) {
-      const int r = BL::kKContig ? (tid >> 3) + 32 * i : tid % BN;
+      const int r = (tid >> 3) + 32 * i;
       const bool ok = n0 + r < N;
       b_off[i] = ok ? b.row_off(n0 + r) : 0;
       b_ok |= (ok ? 1u : 0u) << i;
     }
-    const bool a_vec = a.vec4_ok(), b_vec = b.vec4_ok();
-    constexpr int NVA = kBM * 8 / kProducerThreads, NVB = BN * 8 / kProducerThreads;
-    float4 av[NVA], bv[NVB], an[NVA], bn[NVB];
-    auto gather_a = [&](int64_t k0, float4 (&dst)[NVA]) {
-      if (AL::kKContig) gather_tile<kBM>(a, a_off, a_ok, k0, ke, a_vec, tid, dst);
-      else gather_tile_mn<kBM>(a, m0, M, k0, ke, a_vec, tid, dst);
-    };
-    auto gather_b = [&](int64_t k0, float4 (&dst)[NVB]) {
-      if (BL::kKContig) gather_tile<BN>(b, b_off, b_ok, k0, ke, b_vec, tid, dst);
-      else gather_tile_mn<BN>(b, n0, N, k0, ke, b_vec, tid, dst);
-    };
-    // bias gradient fused into the weight-gradient GEMM: B = dY[k, n] is read by these threads
-    // anyway; in the MN-major gather every chunk of a thread covers the same 4 columns, so one
-    // float4 per thread accumulates the column sums of the CTA's K range.
-    const bool do_colsum = EPI == EPI_ATOMIC && !BL::kKContig && epi.colsum != nullptr &&
-                           blockIdx.y == 0;
-    float4 bsum = make_float4(0.f, 0.f, 0.f, 0.f);
-    const int abl = TC_ABL(g_tc_variant);   // ablation probes (profiles/tc_ablate.py); 0 in production
-    if (nkb > 0) {
-      gather_a(kb, av);
-      gather_b(kb, bv);
-    }
-    // One K block: issue the NEXT block's global loads into `nxt`, then split/store `cur`.
-    // The two register sets swap roles every block (loop unrolled by two below) — copying
-    // nxt -> cur at the end of the body would wait for the loads that were just issued.
-    auto k_block = [&](int kbi, float4 (&cur_a)[NVA], float4 (&cur_b)[NVB], float4 (&nxt_a)[NVA],
-                       float4 (&nxt_b)[NVB]) {
-      const int s = kbi % STAGES;
-      const uint32_t ph = (uint32_t)((kbi / STAGES) & 1);
-      if (kbi + 1 < nkb && abl != 22 && abl != 23 && abl != 24) {
-        const int64_t k1 = kb + (int64_t)(kbi + 1) * kBK;
-        gather_a(k1, nxt_a);
-        gather_b(k1, nxt_b);
-      }
-      if (kbi >= STAGES) mbar_wait(smem_addr(&empty[s]), ph ^ 1u);
-      if (abl == 20 || abl == 23 || abl == 24) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_addr(&full[s]));
-        return;
-      }
-      unsigned char* st = smem + s * L::kStage;
-      unsigned char* a_hi = st;
-      unsigned char* a_lo = st + L::kATile;
-      unsigned char* b_hi = st + L::kNumA * L::kATile;
-      unsigned char* b_lo = b_hi + L::kBTile;
-      if (AL::kKContig) scatter_tile<kBM, kLoA, true>(a_hi, a_lo, tid, cur_a);
-      else scatter_tile_mn<kBM, kLoA>(a_hi, a_lo, tid, cur_a);
-      if (BL::kKContig) scatter_tile<BN, kLo, true>(b_hi, b_lo, tid, cur_b);
-      else scatter_tile_mn<BN, kLo>(b_hi, b_lo, tid, cur_b);
-      if (do_colsum) {
+  }
+  const bool a_vec = a.vec4_ok(), b_vec = b.vec4_ok();
+  constexpr int NVA = kBM * 8 / kThreads, NVB = BN * 8 / kThreads;
+  float4 av[NVA], bv[NVB], an[NVA], bn[NVB];
+  auto gather_a = [&](int64_t k0, float4 (&dst)[NVA]) {
+    if constexpr (AL::kKContig) gather_tile<kBM>(a, a_off, a_ok, k0, ke, a_vec, tid, dst);
+    else gather_tile_mn<kBM>(a, m0, M, k0, ke, a_vec, tid, dst);
+  };
+  auto gather_b = [&](int64_t k0, float4 (&dst)[NVB]) {
+    if constexpr (BL::kKContig) gather_tile<BN>(b, b_off, b_ok, k0, ke, b_vec, tid, dst);
+    else gather_tile_mn<BN>(b, n0, N, k0, ke, b_vec, tid, dst);
+  };
+  // bias gradient fused into the weight-gradient GEMM: B = dY[k, n] is read by these threads
+  // anyway; in the MN-major gather every chunk of a thread covers the same 4 columns, so one
+  // float4 per thread accumulates the column sums of the CTA's K range.
+  const bool do_colsum = EPI == EPI_ATOMIC && !BL::kKContig && epi.colsum != nullptr &&
+                         blockIdx.y == 0;
+  float4 bsum = make_float4(0.f, 0.f, 0.f, 0.f);
+  float acc[BN / 2];
 #pragma unroll
-        for (int i = 0; i < NVB; ++i) {
-          bsum.x += cur_b[i].x; bsum.y += cur_b[i].y; bsum.z += cur_b[i].z; bsum.w += cur_b[i].w;
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  if (nkb > 0) {
+    gather_a(kb, av);
+    gather_b(kb, bv);
+  }
+  const uint32_t smem_base = smem_addr(smem);
+  // One K block: issue the NEXT block's global loads into `nxt`, split/store `cur`, barrier, MMAs.
+  // The two register sets swap roles every block (loop unrolled by two below) -- copying
+  // nxt -> cur at the end of the body would wait for the loads that were just issued.
+  auto k_block = [&](int kbi, float4 (&cur_a)[NVA], float4 (&cur_b)[NVB], float4 (&nxt_a)[NVA],
+                     float4 (&nxt_b)[NVB]) {
+    const int s = kbi % kStages;
+    if (kbi + 1 < nkb) {
+      const int64_t k1 = kb + (int64_t)(kbi + 1) * kBK;
+      gather_a(k1, nxt_a);
+      gather_b(k1, nxt_b);
+    }
+    unsigned char* st = smem + s * L::kStage;
+    unsigned char* a_hi = st;
+    unsigned char* a_lo = st + L::kATile;
+    unsigned char* b_hi = st + L::kNumA * L::kATile;
+    unsigned char* b_lo = b_hi + L::kBTile;
+    if constexpr (AL::kKContig) scatter_tile<kBM, kLoA>(a_hi, a_lo, tid, cur_a);
+    else scatter_tile_mn<kBM, kLoA>(a_hi, a_lo, tid, cur_a);
+    if constexpr (BL::kKContig) scatter_tile<BN, kLo>(b_hi, b_lo, tid, cur_b);
+    else scatter_tile_mn<BN, kLo>(b_hi, b_lo, tid, cur_b);
+    if (do_colsum) {
+#pragma unroll
+      for (int i = 0; i < NVB; ++i) {
+        bsum.x += cur_b[i].x; bsum.y += cur_b[i].y; bsum.z += cur_b[i].z; bsum.w += cur_b[i].w;
+      }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic stores -> async proxy
+    __syncthreads();
+    const uint32_t sa = smem_base + (uint32_t)s * L::kStage + (uint32_t)wg * (64u * 128u);
+    const uint32_t sb = smem_base + (uint32_t)s * L::kStage + L::kNumA * L::kATile;
+    const uint32_t a_lo_off = L::kATile, b_lo_off = L::kBTile;
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < kBK / 8; ++ks) {
+      const uint32_t ko = (uint32_t)ks * 32u;   // 8 tf32 = 32 bytes further inside the 128 B row
+      if (PASSES == 3 && AL::kExact) {
+        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + b_lo_off + ko));
+        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko));
+      } else if (PASSES == 3) {
+        wgmma_tf32<BN>(acc, make_desc(sa + a_lo_off + ko), make_desc(sb + ko));
+        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + b_lo_off + ko));
+        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko));
+      } else {
+        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko));
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+  };
+#pragma unroll 1
+  for (int kbi = 0; kbi < nkb; kbi += 2) {
+    k_block(kbi, av, bv, an, bn);
+    if (kbi + 1 < nkb) k_block(kbi + 1, an, bn, av, bv);
+  }
+  wgmma_wait<0>();
+  if (tid == 0) stamp(2);
+  __syncthreads();   // every MMA of the CTA has retired: the stage buffers hold the staging tile now
+
+  // ===================== epilogue =====================
+  constexpr int P = L::kPitch;
+  float* stg = reinterpret_cast<float*>(smem);
+  {
+    // wgmma m64nNk8 accumulator: register 4i + 2h + e of lane l in warp w (of the warpgroup) is
+    // row 16 w + l / 4 + 8 h, column 8 i + 2 (l % 4) + e
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      *reinterpret_cast<float2*>(stg + r0 * P + 8 * i + c0) = make_float2(acc[4 * i], acc[4 * i + 1]);
+      *reinterpret_cast<float2*>(stg + (r0 + 8) * P + 8 * i + c0) =
+          make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+    }
+  }
+  if (do_colsum) {
+    // thread tid holds columns 4 cm .. 4 cm + 3 (MnMap); the k-lanes of a column are combined
+    // with shared-memory atomics, one red per column goes to global memory
+    const int c4 = MnMap<BN>::cm(tid) * 4;
+    atomicAdd(&sbias[c4 + 0], bsum.x);
+    atomicAdd(&sbias[c4 + 1], bsum.y);
+    atomicAdd(&sbias[c4 + 2], bsum.z);
+    atomicAdd(&sbias[c4 + 3], bsum.w);
+  }
+  // bias slice of this tile -> shared memory
+  if (EPI == EPI_STORE && tid < BN) sbias[tid] = (bias != nullptr && n0 + tid < N) ? bias[n0 + tid] : 0.f;
+  __syncthreads();
+  if (do_colsum && tid < BN && n0 + tid < N) atomicAdd(epi.colsum + n0 + tid, sbias[tid]);
+  if (tid == 0) stamp(4);
+  const int q = warp & 3, half = warp >> 2;   // row quadrant / column half of this warp
+  const int row = q * 32 + lane;
+  const int64_t m = m0 + row;
+  float* out = (splits > 1) ? ws + (int64_t)split * M * N : C;
+  const bool vec_out = (N & 3) == 0 && ((uintptr_t)out & 15) == 0;
+  constexpr int G = 16;  // columns handled per step
+#pragma unroll
+  for (int cc = 0; cc < BN / 2; cc += G) {
+    const int c = half * (BN / 2) + cc;
+    float r[G];
+#pragma unroll
+    for (int j = 0; j < G; j += 4) {
+      const float4 t = *reinterpret_cast<const float4*>(stg + row * P + c + j);
+      r[j] = t.x; r[j + 1] = t.y; r[j + 2] = t.z; r[j + 3] = t.w;
+    }
+    if (m >= M && !(EPI == EPI_STORE && vec_out)) continue;
+    const int64_t nb = n0 + c;
+    if (EPI == EPI_COL2IM) {
+      if (nkb == 0) continue;
+      // pos -> (n, oy, ox); patch index -> (ky, kx*C + c)
+      uint32_t img, rem, oy, ox;
+      epi.g.d_ohow.divmod((uint32_t)m, img, rem);
+      epi.g.d_ow.divmod(rem, oy, ox);
+      const int64_t wc = (int64_t)epi.g.W * epi.g.C;
+      const int64_t in_off = (int64_t)oy * epi.g.stride * wc + (int64_t)ox * epi.g.stride * epi.g.C;
+      float* base = epi.dx + (int64_t)img * epi.g.H * wc + in_off;
+      // act'(X) of the layer that produced the conv input: the scatter-add is linear, so every
+      // contribution is masked on its way out (X is read at the destination index)
+      const float* ybase = epi.mask.y ? epi.mask.y + (int64_t)img * epi.mask.ld + in_off : nullptr;
+#pragma unroll
+      for (int j = 0; j < G; j += 4) {
+        const int64_t kidx = nb + j;
+        if (kidx >= N) break;
+        uint32_t ky, rr;
+        epi.g.d_kwc.divmod((uint32_t)kidx, ky, rr);
+        float* dst = base + (int64_t)ky * wc + rr;
+        float4 v = make_float4(r[j], r[j + 1], r[j + 2], r[j + 3]);
+        if (ybase) {
+          const float4 y = *reinterpret_cast<const float4*>(ybase + (int64_t)ky * wc + rr);
+          v.x = dact(y.x, v.x, epi.mask.act); v.y = dact(y.y, v.y, epi.mask.act);
+          v.z = dact(y.z, v.z, epi.mask.act); v.w = dact(y.w, v.w, epi.mask.act);
         }
+        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x),
+                     "f"(v.y), "f"(v.z), "f"(v.w)
+                     : "memory");
       }
-      // No fence.proxy.async here: it lowers to MEMBAR.ALL.CTA + FENCE.VIEW.ASYNC, and the
-      // MEMBAR would wait for the next block's global loads that are deliberately in flight.
-      // The release-arrive below orders the stores; the MMA thread runs the proxy fence after
-      // its acquire-wait, i.e. on the causality path between these stores and tcgen05.mma.
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_addr(&full[s]));
-    };
-    for (int kbi = 0; kbi < nkb; kbi += 2) {
-      k_block(kbi, av, bv, an, bn);
-      if (kbi + 1 < nkb) k_block(kbi + 1, an, bn, av, bv);
+      continue;
     }
-    // ===================== epilogue =====================
-    if (tid == 0) stamp(2);
-    if (EPI == EPI_ATOMIC && !BL::kKContig && epi.colsum != nullptr && blockIdx.y == 0) {
-      // chunk cm = tid % (BN/4) holds columns 4cm..4cm+3; the 256/(BN/4) k-lanes of a column are
-      // combined with shared-memory atomics, one red per column goes to global memory
-      const int c4 = (tid % (BN / 4)) * 4;
-      atomicAdd(&sbias[c4 + 0], bsum.x);
-      atomicAdd(&sbias[c4 + 1], bsum.y);
-      atomicAdd(&sbias[c4 + 2], bsum.z);
-      atomicAdd(&sbias[c4 + 3], bsum.w);
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (tid < BN && n0 + tid < N) atomicAdd(epi.colsum + n0 + tid, sbias[tid]);
-    }
-    // bias slice of this tile -> shared memory while the last MMAs drain
-    if (EPI == EPI_STORE) {
-      if (tid < BN) sbias[tid] = (bias != nullptr && n0 + tid < N) ? bias[n0 + tid] : 0.f;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-    }
-    mbar_wait(smem_addr(accum), 0u);
-    if (tid == 0) stamp(4);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int q = warp & 3, half = warp >> 2;   // TMEM lane quadrant / column half of this warp
-    const int64_t m = m0 + q * 32 + lane;
-    float* out = (splits > 1) ? ws + (int64_t)split * M * N : C;
-    const bool vec_out = (N & 3) == 0 && ((uintptr_t)out & 15) == 0;
-    constexpr int G = 16;  // columns fetched per tcgen05.ld
-    constexpr int kStagePitch = BN + 4;
-    static_assert(kBM * (BN + 4) * 4 <= STAGES * L::kStage, "epilogue staging tile must fit");
-    // all TMEM loads of this warp's column half are issued before the single wait
-    uint32_t racc[BN / 2];
-#pragma unroll
-    for (int cc = 0; cc < BN / 2; cc += G) {
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * (BN / 2) + cc);
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-          "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-          : "=r"(racc[cc + 0]), "=r"(racc[cc + 1]), "=r"(racc[cc + 2]), "=r"(racc[cc + 3]),
-            "=r"(racc[cc + 4]), "=r"(racc[cc + 5]), "=r"(racc[cc + 6]), "=r"(racc[cc + 7]),
-            "=r"(racc[cc + 8]), "=r"(racc[cc + 9]), "=r"(racc[cc + 10]), "=r"(racc[cc + 11]),
-            "=r"(racc[cc + 12]), "=r"(racc[cc + 13]), "=r"(racc[cc + 14]), "=r"(racc[cc + 15])
-          : "r"(taddr));
-    }
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int cc = 0; cc < BN / 2; cc += G) {
-      const int c = half * (BN / 2) + cc;
-      const uint32_t* r = racc + cc;
-      if (m >= M && !(EPI == EPI_STORE && vec_out)) continue;
-      const int64_t nb = n0 + c;
-      if (EPI == EPI_COL2IM) {
-        if (nkb == 0) continue;
-        // pos -> (n, oy, ox); patch index -> (ky, kx*C + c)
-        uint32_t img, rem, oy, ox;
-        epi.g.d_ohow.divmod((uint32_t)m, img, rem);
-        epi.g.d_ow.divmod(rem, oy, ox);
-        const int64_t wc = (int64_t)epi.g.W * epi.g.C;
-        const int64_t in_off = (int64_t)oy * epi.g.stride * wc + (int64_t)ox * epi.g.stride * epi.g.C;
-        float* base = epi.dx + (int64_t)img * epi.g.H * wc + in_off;
-        // act'(X) of the layer that produced the conv input: the scatter-add is linear, so every
-        // contribution is masked on its way out (X is read at the destination index)
-        const float* ybase = epi.mask.y ? epi.mask.y + (int64_t)img * epi.mask.ld + in_off : nullptr;
-#pragma unroll
-        for (int j = 0; j < G; j += 4) {
-          const int64_t kidx = nb + j;
-          if (kidx >= N) break;
-          uint32_t ky, rr;
-          epi.g.d_kwc.divmod((uint32_t)kidx, ky, rr);
-          float* dst = base + (int64_t)ky * wc + rr;
-          float4 v = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                 __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-          if (ybase) {
-            const float4 y = *reinterpret_cast<const float4*>(ybase + (int64_t)ky * wc + rr);
-            v.x = dact(y.x, v.x, epi.mask.act); v.y = dact(y.y, v.y, epi.mask.act);
-            v.z = dact(y.z, v.z, epi.mask.act); v.w = dact(y.w, v.w, epi.mask.act);
-          }
-          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x),
-                       "f"(v.y), "f"(v.z), "f"(v.w)
-                       : "memory");
-        }
-        continue;
-      }
-      if (EPI == EPI_ATOMIC) {
-        if (nkb == 0) continue;
-        float* dst = C + m * N + nb;
-        if ((N & 3) == 0 && nb + G - 1 < N) {
-#pragma unroll
-          for (int j = 0; j < G; j += 4)
-            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j),
-                         "f"(__uint_as_float(r[j]) * out_scale), "f"(__uint_as_float(r[j + 1]) * out_scale),
-                         "f"(__uint_as_float(r[j + 2]) * out_scale), "f"(__uint_as_float(r[j + 3]) * out_scale)
-                         : "memory");
-        } else {
-#pragma unroll
-          for (int j = 0; j < G; ++j)
-            if (nb + j < N) atomicAdd(dst + j, __uint_as_float(r[j]) * out_scale);
-        }
-        continue;
-      }
-      float v[G];
-#pragma unroll
-      for (int j = 0; j < G; ++j) {
-        float x = nkb > 0 ? __uint_as_float(r[j]) * out_scale : 0.f;
-        if (splits == 1 && nb + j < N && m < M) {
-          x += sbias[c + j];
-          x = apply_act(x, act);
-          if (!vec_out && epi.mask.y) x = dact(epi.mask.y[m * epi.mask.ld + nb + j], x, epi.mask.act);
-          if (beta) x += out[m * N + nb + j];
-        }
-        v[j] = x;
-      }
-      if (vec_out) {
-        // stage the tile in the (now idle) operand buffers so that global rows are written by
-        // adjacent lanes; row pitch BN+4 floats keeps the 16-byte stores conflict-free
-        float* srow = reinterpret_cast<float*>(smem) + (q * 32 + lane) * kStagePitch + c;
+    if (EPI == EPI_ATOMIC) {
+      if (nkb == 0) continue;
+      float* dst = C + m * N + nb;
+      if ((N & 3) == 0 && nb + G - 1 < N) {
 #pragma unroll
         for (int j = 0; j < G; j += 4)
-          *reinterpret_cast<float4*>(srow + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j),
+                       "f"(r[j] * out_scale), "f"(r[j + 1] * out_scale),
+                       "f"(r[j + 2] * out_scale), "f"(r[j + 3] * out_scale)
+                       : "memory");
       } else {
 #pragma unroll
         for (int j = 0; j < G; ++j)
-          if (nb + j < N) out[m * N + nb + j] = v[j];
+          if (nb + j < N) atomicAdd(dst + j, r[j] * out_scale);
       }
+      continue;
     }
-    if (EPI == EPI_STORE && vec_out) {
-      asm volatile("bar.sync 1, 256;" ::: "memory");   // the 8 epilogue warps only
-      constexpr int LPR = BN / 4;                        // lanes per tile row
-      constexpr int RPI = 32 / LPR;                      // rows per store instruction
-      const int col = (lane % LPR) * 4;
-#pragma unroll 4
-      for (int rr = 0; rr < 16; rr += RPI) {
-        const int row = warp * 16 + rr + lane / LPR;
-        const int64_t gm = m0 + row;
-        if (gm < M && n0 + col < N) {
-          float4 t = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(smem) +
-                                                      row * kStagePitch + col);
-          if (splits == 1 && epi.mask.y) {   // coalesced read of the producing layer's output
-            const float* yp = epi.mask.y + gm * epi.mask.ld + n0 + col;
-            const bool yv = (epi.mask.ld & 3) == 0 && ((uintptr_t)epi.mask.y & 15) == 0;
-            const float4 y = yv ? *reinterpret_cast<const float4*>(yp)
-                                : make_float4(yp[0], yp[1], yp[2], yp[3]);
-            t.x = dact(y.x, t.x, epi.mask.act); t.y = dact(y.y, t.y, epi.mask.act);
-            t.z = dact(y.z, t.z, epi.mask.act); t.w = dact(y.w, t.w, epi.mask.act);
-          }
-          *reinterpret_cast<float4*>(out + gm * N + n0 + col) = t;
-        }
-      }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    if (tid == 0) stamp(5);
-  } else {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(BN, !AL::kKContig, !BL::kKContig);
-      for (int kbi = 0; kbi < nkb; ++kbi) {
-        const int s = kbi % STAGES;
-        const uint32_t ph = (uint32_t)((kbi / STAGES) & 1);
-        mbar_wait(smem_addr(&full[s]), ph);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic stores -> async proxy
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        unsigned char* st = smem + s * L::kStage;
-        const uint32_t a_hi = smem_addr(st), a_lo = a_hi + L::kATile;
-        const uint32_t b_hi = a_hi + L::kNumA * L::kATile, b_lo = b_hi + L::kBTile;
+    float v[G];
 #pragma unroll
-        for (int ks = 0; ks < kBK / 8; ++ks) {
-          // K-major: 8 tf32 = 32 bytes further inside the 128 B row; MN-major: next 8-row k group
-          // K-major: 8 tf32 = 32 B further in the row; MN-major: two 4-row k atoms further
-          const uint32_t ka = AL::kKContig ? (uint32_t)ks * 32u : (uint32_t)ks * 2u * (kBM / 32) * 512u;
-          const uint32_t kbo = BL::kKContig ? (uint32_t)ks * 32u : (uint32_t)ks * 2u * (BN / 32) * 512u;
-          // (the 8-row-atom experiment has the same per-K-step advance: (ROWS/32) * 1024)
-          auto da = [&](uint32_t base) { return AL::kKContig ? make_desc(base + ka) : make_desc_mn(base + ka, (kBM / 32) * 512u); };
-          auto db = [&](uint32_t base) { return BL::kKContig ? make_desc(base + kbo) : make_desc_mn(base + kbo, (BN / 32) * 512u); };
-          const uint32_t first = (kbi == 0 && ks == 0) ? 0u : 1u;
-          if ((TC_ABL(g_tc_variant) == 21 || TC_ABL(g_tc_variant) == 24) && !(kbi == 0 && ks == 0)) continue;
-          if (PASSES == 3 && AL::kExact) {
-            tc_mma_tf32(tmem_base, da(a_hi), db(b_lo), idesc, first);
-            tc_mma_tf32(tmem_base, da(a_hi), db(b_hi), idesc, 1u);
-          } else if (PASSES == 3) {
-            tc_mma_tf32(tmem_base, da(a_lo), db(b_hi), idesc, first);
-            tc_mma_tf32(tmem_base, da(a_hi), db(b_lo), idesc, 1u);
-            tc_mma_tf32(tmem_base, da(a_hi), db(b_hi), idesc, 1u);
-          } else {
-            tc_mma_tf32(tmem_base, da(a_hi), db(b_hi), idesc, first);
-          }
-        }
-        tc_commit(smem_addr(&empty[s]));
+    for (int j = 0; j < G; ++j) {
+      float x = nkb > 0 ? r[j] * out_scale : 0.f;
+      if (splits == 1 && nb + j < N && m < M) {
+        x += sbias[c + j];
+        x = apply_act(x, act);
+        if (!vec_out && epi.mask.y) x = dact(epi.mask.y[m * epi.mask.ld + nb + j], x, epi.mask.act);
+        if (beta) x += out[m * N + nb + j];
       }
-      tc_commit(smem_addr(accum));
-      stamp(3);
+      v[j] = x;
     }
-    __syncwarp();
+    if (vec_out) {
+      // back into the staging row (this thread's own cells) so that global rows are written by
+      // adjacent lanes below; row pitch BN+4 floats keeps the 16-byte accesses conflict-free
+      float* srow = stg + row * P + c;
+#pragma unroll
+      for (int j = 0; j < G; j += 4)
+        *reinterpret_cast<float4*>(srow + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < G; ++j)
+        if (nb + j < N) out[m * N + nb + j] = v[j];
+    }
   }
-  __syncthreads();
-  if (warp == 8) {
-    constexpr int kCols = BN < 32 ? 32 : BN;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "n"(kCols));
-    if (lane == 0) stamp(6);
+  if (EPI == EPI_STORE && vec_out) {
+    __syncthreads();
+    constexpr int LPR = BN / 4;                        // lanes per tile row
+    constexpr int RPI = 32 / LPR;                      // rows per store instruction
+    const int col = (lane % LPR) * 4;
+#pragma unroll 4
+    for (int rr = 0; rr < 16; rr += RPI) {
+      const int srow = warp * 16 + rr + lane / LPR;
+      const int64_t gm = m0 + srow;
+      if (gm < M && n0 + col < N) {
+        float4 t = *reinterpret_cast<const float4*>(stg + srow * P + col);
+        if (splits == 1 && epi.mask.y) {   // coalesced read of the producing layer's output
+          const float* yp = epi.mask.y + gm * epi.mask.ld + n0 + col;
+          const bool yv = (epi.mask.ld & 3) == 0 && ((uintptr_t)epi.mask.y & 15) == 0;
+          const float4 y = yv ? *reinterpret_cast<const float4*>(yp)
+                              : make_float4(yp[0], yp[1], yp[2], yp[3]);
+          t.x = dact(y.x, t.x, epi.mask.act); t.y = dact(y.y, t.y, epi.mask.act);
+          t.z = dact(y.z, t.z, epi.mask.act); t.w = dact(y.w, t.w, epi.mask.act);
+        }
+        *reinterpret_cast<float4*>(out + gm * N + n0 + col) = t;
+      }
+    }
   }
+  if (tid == 0) stamp(5);
 }
 
 }  // namespace tc

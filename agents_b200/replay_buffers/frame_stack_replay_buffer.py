@@ -14,7 +14,7 @@ predecessors afterwards, so a rebuilt stack never reads an overwritten slot; Buf
 probability of that range.
 Everything else (ring layout, Philox draws, BufferInfo) is the wrapped TFUniformReplayBuffer.
 
-Validated on a B200 (tests/test_zz_late_gpu.py: rebuilt stacks are bit-identical to what a
+Validated on the GPU (tests/test_zz_late_gpu.py: rebuilt stacks are bit-identical to what a
 FrameStack-K producer emitted, before and after the ring wraps).
 """
 import ctypes

@@ -5,7 +5,7 @@ The reference's `ReverbReplayBuffer` / `Reverb*Observer` classes
 external `dm-reverb` gRPC server through three objects: a *trajectory writer* (`append` one step,
 `history[-n:]` column slices, `create_item(table, trajectory, priority)`, `end_episode`), a
 *table* (sampler, remover, `max_size`, `max_times_sampled`, rate limiter) and a *client*
-(`server_info`, `reset`, `mutate_priorities`).  dm-reverb is not part of `/root/reference`
+(`server_info`, `reset`, `mutate_priorities`).  dm-reverb is not part of the reference repository
 (go.mod-style external dependency, un-vendored), so this module restates that model — the format
 in which the observers hand data over — as a single-process server whose payload lives on the GPU:
 

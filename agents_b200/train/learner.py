@@ -16,7 +16,6 @@ import os
 
 import torch
 
-from agents_b200 import _lib
 from agents_b200.agents import tf_agent
 from agents_b200.train.utils import strategy_utils
 from agents_b200.utils import nest
@@ -101,9 +100,6 @@ class Learner(object):
     if n > 1:
       agent.replicas = n
       agent._grad_sync = self.strategy.all_reduce_sum
-      if torch.cuda.is_available() and os.environ.get('B200RL_TILE_SCHED') is None:
-        # the bucketed gradient all-reduce shares the SMs with the backward GEMMs
-        _lib.call('b200rl_set_tile_scheduler', 1)
       if hasattr(agent, '_stat_sync'):
         agent._stat_sync = self.strategy.all_reduce_sum
         agent._replica_rank = self.strategy.rank

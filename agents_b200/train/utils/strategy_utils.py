@@ -77,7 +77,7 @@ def get_strategy(tpu=None, use_gpu=True):
   """Returns the strategy for this process (strategy_utils.py:36-61): the process-group
   strategy when launched under torchrun with WORLD_SIZE > 1, else the single-replica default."""
   if tpu:
-    raise NotImplementedError('TPUStrategy has no B200 equivalent.')
+    raise NotImplementedError('TPUStrategy has no CUDA equivalent.')
   if dist.is_initialized() and dist.get_world_size() > 1:
     return ProcessGroupStrategy()
   if int(os.environ.get('WORLD_SIZE', '1')) > 1 and not dist.is_initialized():

@@ -1,4 +1,4 @@
-"""bench.py — train steps/sec (DQN Atari-shape, batch 256) on N B200s, replay GB/s.
+"""bench.py — train steps/sec (DQN Atari-shape, batch 256) on N H100s, replay GB/s.
 
 Workload (BASELINE.json configs[1]): synthetic Atari-shape observations 84x84x4 uint8, a
 1 048 576-slot TFUniformReplayBuffer (256 segments x 4096) per GPU, sample batch 256 x T=2,
@@ -6,8 +6,13 @@ Mnih'15 Q-network, Huber loss, centered RMSProp (examples/dqn/mnih15 config), ga
 target update every 2500 steps.  One "step" = get_next(256, 2) + DqnAgent.train(experience).
 
   value        steps/s with the ring resident in HBM; the step is replayed as ONE CUDA graph.
-               `--steps K` steps are timed `--repeats R` times (each block bracketed by
-               barrier + synchronize, CUDA events, max over ranks); value is the MEDIAN block.
+               Exactly `--steps K` steps are timed, split into `--repeats R` blocks (each block
+               bracketed by barrier + synchronize, CUDA events, max over ranks); value is the
+               MEDIAN block rate.
+  --dump-outputs DIR   after the timed steps, writes what the last timed step returned to its
+               caller (loss, the updated Q-network parameters, the sampled batch; a fixed seeded
+               sample of the observations) as DIR/<name>.npy in float32 / float64.  Inputs are
+               seeded, so two builds run with the same arguments can be compared file by file.
   e2e          the same step through the public API with HOST buffers: every step copies one
                driver step of collected frames (256 x 28 244 B) from pinned host memory,
                add_batch, get_next, train, and reads that step's loss back (the read of step
@@ -63,7 +68,8 @@ def _peaks():
     d = json.load(open(p))
     return dict(hbm=d['hbm_gbs'], tensor_burst=d['bf16_tflops'],
                 tensor=d.get('bf16_tflops_sustained', d['bf16_tflops']), src='measured')
-  return dict(hbm=6650.0, tensor_burst=1590.0, tensor=1400.0, src='fallback')
+  # H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16
+  return dict(hbm=3350.0, tensor_burst=989.0, tensor=989.0, src='H100 SXM data sheet')
 
 
 def _mnih_layers(rng):
@@ -275,6 +281,27 @@ def _oracle_layers(net, Ly):
   return layers
 
 
+def _dump_outputs(out_dir, loss, net, exp):
+  """Writes the last timed step's results as float32 / float64 .npy files (well under 64 MB)."""
+  import torch
+  os.makedirs(out_dir, exist_ok=True)
+
+  def save(name, t, dtype):
+    np.save(os.path.join(out_dir, name + '.npy'), t.detach().cpu().numpy().astype(dtype))
+
+  save('loss', loss.reshape(1), np.float32)
+  save('q_network_params', net.flat_params, np.float32)
+  if exp is not None:
+    save('step_type', exp.step_type, np.float64)
+    save('action', exp.action, np.float64)
+    save('reward', exp.reward, np.float32)
+    save('discount', exp.discount, np.float32)
+    obs = exp.observation.reshape(-1)
+    g = torch.Generator(device=obs.device).manual_seed(0)
+    idx = torch.randint(0, obs.numel(), (1 << 20,), device=obs.device, generator=g)
+    save('observation_sample', obs[idx], np.float32)
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--gpus', type=int, default=1)
@@ -290,6 +317,8 @@ def main():
   ap.add_argument('--no-prefetch', action='store_true',
                   help='sample and train back to back on one stream (default: the sample of step '
                        'i+1 runs on a side stream beside train(i), like dataset.prefetch(1))')
+  ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                  help='write the outputs of the last timed step to DIR/<name>.npy')
   ap.add_argument('--ncu-step', action='store_true',
                   help='after warm-up run ONE un-captured step between cudaProfilerStart/Stop and '
                        'exit (target of `ncu --profile-from-start off`; prints no bench value)')
@@ -324,7 +353,9 @@ def main():
   strategy = strategy_utils.get_strategy()
   W = max(args.warmup, 3)
   K = args.steps
-  R = max(1, args.repeats)
+  K = max(1, K)
+  R = max(1, min(args.repeats, K))
+  block_steps = [K // R + (1 if i < K % R else 0) for i in range(R)]   # sums to K
   peaks = _peaks()
   extra = {}
 
@@ -488,16 +519,16 @@ def main():
       print(json.dumps({'ncu_step': True, 'launches_per_step': launches_per_step}))
     return
 
-  # ---- timed region: R blocks of K steps, CUDA events, max over ranks, median block -------------
+  # ---- timed region: K steps in R blocks, CUDA events, max over ranks, median block rate ---------
   clocks = ClockSampler(local_rank)
   clocks.start()
   block_ms = []
   t_wall0 = time.perf_counter()
-  for _ in range(R):
+  for n_steps in block_steps:
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     sync_all()
     e0.record()
-    for _ in range(K):
+    for _ in range(n_steps):
       loss = fn()
     e1.record()
     sync_all()
@@ -507,16 +538,19 @@ def main():
       dist.all_reduce(t, op=dist.ReduceOp.MAX)
       ms = float(t.item())
     block_ms.append(ms)
+  if args.dump_outputs and rank == 0:
+    _dump_outputs(args.dump_outputs, loss, net,
+                  sample_bufs[(step_no[0] - 1) & 1][0] if prefetch else None)
   # keep the sampler running over a load of at least ~1.5 s so that it sees the step's clocks
   while time.perf_counter() - t_wall0 < 1.5:
     for _ in range(K):
       fn()
     torch.cuda.synchronize()
   clk = clocks.stop()
-  ms = float(np.median(block_ms))
+  ms_step = float(np.median([b / n for b, n in zip(block_ms, block_steps)]))
   final_loss = float(loss.item())
   agent.check_numerics()
-  steps_per_s = K / (ms / 1000.0)
+  steps_per_s = 1000.0 / ms_step
   value = steps_per_s * world                  # batch-256-equivalent steps/s of the whole job
 
   # ---- per-kernel timing for the rooflines (CUDA events on the launch stream) -------------------
@@ -664,8 +698,8 @@ def main():
   if rank == 0:
     line = dict(
         metric='train steps/sec (DQN Atari-shape, batch 256)', value=value, unit='steps/s',
-        n_gpus=world, steps=K, warmup=W, repeats=R, ms_per_step=ms / K,
-        block_ms=[round(b, 4) for b in block_ms], higher_is_better=True,
+        n_gpus=world, steps=K, warmup=W, repeats=R, ms_per_step=ms_step,
+        block_ms=[round(b, 4) for b in block_ms], block_steps=block_steps, higher_is_better=True,
         scaling='weak', vs_baseline=None, dtype='f32 (3xTF32 tensor-core GEMMs, fp32 accumulate)', data='synthetic',
         config=dict(workload=WORKLOAD, global_batch=B * world, per_gpu_batch=B, num_actions=A,
                     parallelism=f'dp{world}' if world > 1 else 'single',
@@ -677,8 +711,8 @@ def main():
                     cuda_graph=bool(use_graph), collect_frames_per_e2e_step=B_ENV,
                     input_pipeline=('prefetch(1): sample of step i+1 on a side stream beside train(i), two '
                                     'sample buffers' if prefetch else 'sample then train on one stream'),
-                    timing=f'median of {R} blocks of {K} graph replays, each block bracketed by '
-                           'barrier + synchronize, CUDA events, max over ranks',
+                    timing=f'{K} graph replays in {R} blocks, median block rate; each block bracketed '
+                           'by barrier + synchronize, CUDA events, max over ranks',
                     e2e_pipeline='pinned host frames -> double-buffered H2D on a copy stream -> '
                                  'common.function(add_batch + get_next + train) per staging slot -> per-step loss '
                                  'D2H into pinned slots, read one step behind'),
@@ -686,10 +720,10 @@ def main():
         e2e=dict(value=e2e_value, unit='steps/s', h2d_bytes_per_step=h2d, d2h_bytes_per_step=4,
                  steps=Ke, losses_read=len(losses_read)),
         gpu_launches=int(launches_per_step * K),
-        roofline=dict(kernel='tc2_gemm_kernel / tc_gemm_kernel (Q-net conv/dense fwd+bwd, tcgen05 kind::tf32, 3xTF32)', bound='tensor',
+        roofline=dict(kernel='tc_gemm_kernel (Q-net conv/dense fwd+bwd, wgmma tf32, 3xTF32)', bound='tensor',
                       achieved=update_tfs, peak=peaks['tensor'], unit='TFLOP/s',
                       frac=update_tfs / peaks['tensor'], traffic=traffic.get('update'),
-                      peak_source=peaks['src'] + ' bf16 sustained', ms=update_ms,
+                      peak_source=peaks['src'] + ' bf16', ms=update_ms,
                       algorithmic_flops=FLOPS_PER_STEP,
                       # fp32-equivalent ceiling of the arithmetic actually used: TF32 runs at half
                       # the bf16 rate and 3xTF32 issues three MMAs per product -> peak / 6
@@ -742,7 +776,7 @@ def main():
   if not args.no_extra:
     from profiles import configs
     guarded('gather_sweep', lambda: configs.gather_sweep(
-        dev, world, rank, peaks, caps_m=(1, 2, 4) if world == 1 else ((1, 4, 8) if world == 2 else (1, 4, 8, 16))))
+        dev, world, rank, peaks, caps_m=(1, 2) if world == 1 else ((1, 2, 4) if world == 2 else (1, 4, 8))))
     guarded('ppo_update', lambda: configs.ppo_update(strategy, dev, peaks))
     guarded('sac_step', lambda: configs.sac_step(strategy, dev, peaks))
     if world == 1:

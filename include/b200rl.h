@@ -1,12 +1,12 @@
 /*
  * b200rl.h — C ABI of libb200rl.so: the collect -> store -> sample -> update hot path
- * of TF-Agents, as hand-written sm_100a CUDA.
+ * of TF-Agents, as hand-written sm_90a (H100) CUDA.
  *
  * The reference (tensorflow/agents @ eb24cf5f) has no FFI for this path: it is plain
  * Python over TensorFlow ops (SURVEY.md §8b).  This header therefore *defines* the
  * boundary a reference maintainer would bind with ctypes (see INTEGRATION.md); every
  * entry point cites the reference function whose device work it replaces.  All
- * file:line citations are relative to /root/reference/tf_agents/.
+ * file:line citations are relative to tf_agents/ in the reference repository.
  *
  * Conventions
  *   - Every pointer named *_dev / documented "device" is a CUDA device pointer owned by the
@@ -341,30 +341,14 @@ int b200rl_concat2(const float* a, int64_t lda, int64_t da, const float* b, int6
  * All matrices are row-major.
  * ------------------------------------------------------------------------------------ */
 /* GEMM engine for every dense / conv entry point below: 0 = fp32 FFMA register-tiled kernel,
- * 1 = tcgen05 tensor cores with the 3xTF32 split (fp32-grade accuracy, TMEM accumulators),
- * 2 = tcgen05 single-pass TF32 (~1e-3 relative; NOT within the 1e-5 parity bar).
+ * 1 = Hopper wgmma tensor cores with the 3xTF32 split (fp32-grade accuracy, fp32 accumulators),
+ * 2 = wgmma single-pass TF32 (~1e-3 relative; NOT within the 1e-5 parity bar).
  * Default: env B200RL_GEMM_MODE, else 1.  Outputs narrower than 16 columns (Q head, value head)
  * always use mode 0. */
 int b200rl_set_gemm_mode(int mode);
 /* Profiling aid: device buffer of int64[64][8] that receives %globaltimer phase stamps of the
- * first 64 CTAs of every tcgen05 GEMM launch (NULL disables). */
+ * first 64 CTAs of every tensor-core GEMM launch (NULL disables). */
 int b200rl_tc_debug_buffer(long long* dev_buf);
-/* Profiling/bring-up aid: selects an MN-major tile layout experiment (0 = production). */
-int b200rl_tc_debug_variant(int v);
-/* Second-generation GEMM kernel (tc2_gemm.cuh) switches.  bit 0: store an explicitly masked
- * TF32 "hi" plane instead of using the raw fp32 operand tile for it (the tensor core ignores the
- * low 13 mantissa bits; both settings are bit-identical, the default saves the store).  bit 1 (or B200RL_TC2=0 in the environment): route every GEMM to the
- * first-generation kernel (A/B comparisons in profiles/tc2_check.py).  bit 2: load plain 2-D
- * operands with cp.async like the im2col views instead of TMA tensor tiles. */
-int b200rl_set_tc2_flags(int flags);
-/* Work distribution of the persistent tcgen05 GEMM: 0 (default) static striding over the CTAs,
- * 1 dynamic (global tile counter) -- set by the data-parallel Learner (train/learner.py:104-143 in
- * the reference is where the strategy is attached) so that CTAs whose SM is held by the gradient
- * all-reduce take fewer tiles; B200RL_TILE_SCHED=0/1 in the environment sets the initial value. */
-int b200rl_set_tile_scheduler(int dynamic);
-/* Profiling aid: CTA 0 of every tc2 GEMM stamps %globaltimer at the start/end of each pipeline
- * step of each role into dev_buf[4 roles][256 steps][2] (int64); NULL switches it off. */
-int b200rl_tc2_trace_buffer(long long* dev_buf);
 
 /* Y[M,N] = act(X[M,K] @ W[K,N] + bias[N]).  ldx = row stride of X in elements (0 -> K), so a
  * [B,T,K] batch can be read at a fixed t without a copy.  workspace: device scratch of

@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY.  Nothing under agents_b200/ imports this package; only tests/,
 __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may.  Every
-function cites the reference file:line (relative to /root/reference/tf_agents/) it restates.
+function cites the reference file:line (relative to tf_agents/ in the reference repository) it restates.
 
 Pinning status (SURVEY.md §8c): ring / window / probability semantics, n-step, returns, GAE,
 Q indexing, Polyak, Periodically, DQN/PPO/SAC scalar losses are pinned against the reference's

@@ -4,7 +4,7 @@
 The reference stores Atari observations as 4-frame stacks `[84, 84, 4]` in
 `TFUniformReplayBuffer` and offers frame de-duplication only in the host-side
 `PyHashedReplayBuffer` (replay_buffers/py_hashed_replay_buffer.py:37-181: frames are hashed,
-each unique frame is stored once and stacks are rebuilt on sampling).  The B200 plan keeps the
+each unique frame is stored once and stacks are rebuilt on sampling).  The CUDA plan keeps the
 ring of `oracle/replay.py` but stores ONE frame per slot and rebuilds the stack in the gather
 kernel.  This module fixes the semantics that kernel must reproduce:
 

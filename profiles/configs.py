@@ -238,7 +238,7 @@ def cartpole_iter(dev, iters=2000):
 
 
 # ---- config 5 ------------------------------------------------------------------------------------
-def gather_sweep(dev, world, rank, peaks, caps_m=(1, 2, 4), batches=(64, 256, 1024, 4096), T=2,
+def gather_sweep(dev, world, rank, peaks, caps_m=(1, 2), batches=(64, 256, 1024, 4096), T=2,
                  nl=20, reps=5):
   """b200rl_rb_sample on Atari-shape rows.  `caps_m` are GLOBAL capacities in Mi slots; each rank
   owns capacity/world of it (shard by segment, no exchange) and samples batch/world windows, so
@@ -398,8 +398,8 @@ if __name__ == '__main__':
     dist.init_process_group('nccl', device_id=dev)
   strategy = strategy_utils.get_strategy()
   pk = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json'))) if os.path.exists(
-      os.path.join(ROOT, 'MEASURED_PEAKS.json')) else dict(hbm_gbs=6650.0, bf16_tflops_sustained=1400.0)
-  peaks = dict(hbm=pk['hbm_gbs'], tensor=pk.get('bf16_tflops_sustained', pk.get('bf16_tflops', 1400.0)))
+      os.path.join(ROOT, 'MEASURED_PEAKS.json')) else dict(hbm_gbs=3350.0, bf16_tflops_sustained=989.0)   # H100 SXM data sheet
+  peaks = dict(hbm=pk['hbm_gbs'], tensor=pk.get('bf16_tflops_sustained', pk.get('bf16_tflops', 989.0)))
   res = dict(ppo=lambda: ppo_update(strategy, dev, peaks), sac=lambda: sac_step(strategy, dev, peaks),
              cartpole=lambda: cartpole_iter(dev),
              gather=lambda: gather_sweep(dev, world, strategy.rank, peaks),

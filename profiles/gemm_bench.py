@@ -1,5 +1,5 @@
 """Q-network GEMM micro-benchmark: Mnih'15 net at batch 256, forward (+tape) and backward, per
-GEMM engine (0 = fp32 FFMA, 1 = tcgen05 3xTF32, 2 = tcgen05 1xTF32).  CUDA events, 20 reps.
+GEMM engine (0 = fp32 FFMA, 1 = wgmma 3xTF32, 2 = wgmma 1xTF32).  CUDA events, 20 reps.
 Usage: python profiles/gemm_bench.py [--modes 0,1] [--reps 20] [--layer conv2]"""
 import argparse
 import json

@@ -1,7 +1,7 @@
 """Per-layer GEMM timing of the Mnih'15 Q-network at batch 256 (config 2 shapes): forward, input
 gradient (dX) and parameter gradient (dW + db) of every layer, each timed as R back-to-back
 launches replayed from one CUDA graph (CUDA events on the launch stream; the number is kernel
-time, not Python launch overhead), plus the %globaltimer phase stamps of the tcgen05 kernel.
+time, not Python launch overhead), plus the %globaltimer phase stamps of the tensor-core kernel.
 
     python profiles/layer_probe.py [--reps 20] [--batch 256] [--stamps]
 

@@ -1,9 +1,5 @@
 """One forward_train + backward of the Mnih'15 Q-network (batch 256) between cudaProfilerStart /
-cudaProfilerStop, after two warm-up passes -- the target of the ncu captures:
-
-    ncu --set full --clock-control none --import-source on --profile-from-start off \
-        -k regex:tc_gemm -o gpurun_out/r2_net python profiles/net_once.py
-"""
+cudaProfilerStop, after two warm-up passes -- a target for a profiler that honours those calls."""
 import os
 import sys
 

@@ -12,7 +12,7 @@ if HERE not in sys.path:
 
 
 def pytest_configure(config):
-  config.addinivalue_line('markers', 'gpu: test needs a CUDA device (run on the B200 box)')
+  config.addinivalue_line('markers', 'gpu: test needs a CUDA device (an H100)')
 
 
 @pytest.fixture(scope='session')

@@ -3,7 +3,7 @@
 The layer- and kernel-level tests run small shapes; these run >= 3 complete train steps at the
 benchmark shapes and compare loss / per-example td_error / post-step parameters with the oracle:
 
-  config 2  Mnih'15 Q-net, batch 256, T=2, centered RMSProp, tcgen05 3xTF32 path end to end
+  config 2  Mnih'15 Q-net, batch 256, T=2, centered RMSProp, wgmma 3xTF32 path end to end
             (oracle/dqn_torch.py, cross-checked against oracle/dqn.py in tests/test_oracle_nn.py)
   config 3  PPO (200, 100) tanh nets, T=128, both normalisers ON, 2 epochs x 2 train calls; the
             4096 trajectories are cut to 512 so that the numpy oracle stays within seconds
@@ -123,7 +123,7 @@ def test_config2_dqn_mnih_batch256_train_parity(cuda):
 
 def test_dqn_train_parity_all_layers_on_tensor_cores(cuda):
   """5 steps of a conv net whose every layer has >= 16 output channels at batch 32, so conv1 also
-  takes the tcgen05 path (numpy oracle, Adam, n-step 2, clipping, Polyak)."""
+  takes the tensor-core path (numpy oracle, Adam, n-step 2, clipping, Polyak)."""
   rng = np.random.RandomState(3)
   A, B, n = 4, 32, 2
   obs_spec = tensor_spec.TensorSpec((28, 28, 4), torch.uint8)
@@ -259,8 +259,7 @@ def test_config4_sac_256x256_batch1024_train_parity(cuda):
     np.testing.assert_allclose(got.loss.item(), want['loss'], rtol=1e-5, atol=5e-5)
   # Adam divides by sqrt(v): where a gradient element is ~0 (dead ReLU paths) a 1e-9 difference
   # in g moves the parameter by up to lr per step, so parameters are compared as "all but a
-  # vanishing fraction within 1e-3 relative, none further than steps * lr" (measured on B200:
-  # 8 of 65 536 actor weights beyond the tight bound, max 5.2e-4)
+  # vanishing fraction within 1e-3 relative, none further than steps * lr"
   bad, total, worst_abs = 0, 0, 0.0
   for v, w in zip(actor.variables, orc.actor.params()):
     g = v.cpu().numpy()

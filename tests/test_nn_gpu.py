@@ -20,10 +20,7 @@ def _close(got, want, rtol=2e-5, atol=None, tag=None):
   3xTF32 drops the lo*lo term (2^-22 per product), so single ELEMENTS of a cancelling sum differ by
   up to ~1e-4 of their own value while the error relative to the largest element stays near 1e-6;
   that figure is recorded per tag (gpurun_out/parity_measured.json -> profiles/) and the loss-level
-  1e-5 bound of the north star is asserted in tests/test_baseline_parity_gpu.py.  Measured on B200
-  (profiles/r2/run23_parity_measured.json, worst case over all shapes): dense dW 2.1e-6, dX 1.9e-6,
-  db 4.9e-6; conv dW 2.0e-6, dX 7.1e-7, db 1.5e-6; the whole Mnih net's gradients 3.0e-6 -- all
-  below 1e-5 of the largest element."""
+  1e-5 bound of the north star is asserted in tests/test_baseline_parity_gpu.py."""
   want = np.asarray(want)
   if atol is None:
     atol = 2e-6 * max(1.0, float(np.abs(want).max()))

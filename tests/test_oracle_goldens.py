@@ -1,7 +1,7 @@
 """Pins the CPU oracle to the reference's own test goldens (SURVEY.md §8c).
 
 Each test names the reference test it replays (paths relative to
-/root/reference/tf_agents/).  No GPU, no reference import: the literals below are the
+tf_agents/ in the reference repository).  No GPU, no reference import: the literals below are the
 reference's expected values.
 """
 import numpy as np

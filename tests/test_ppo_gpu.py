@@ -201,10 +201,8 @@ def test_ppo_clip_agent_train_parity(cuda, cfg):
     infos = orc.train(e)
     got = agent.train(_to_traj(cuda, e))
     want = infos[-1]
-    # north-star bound 1e-5 relative on every loss term.  Measured on B200 (run 23,
-    # profiles/r2/run23_parity_measured.json, worst of both configs and all calls): total loss
-    # 2.3e-7, policy-gradient loss 1.1e-6 relative (2.5e-7 absolute; it is a mean of ratio * advantage
-    # terms of both signs, hence the absolute floor), post-Adam parameters 1.9e-6 absolute.
+    # north-star bound 1e-5 relative on every loss term (the policy-gradient loss is a mean of
+    # ratio * advantage terms of both signs, hence an absolute floor as well).
     record_parity('ppo_train_b64_t33', loss_rel=abs(got.loss.item() - want['loss']) / max(abs(want['loss']), 1e-30),
                   pg_abs=abs(got.extra.policy_gradient_loss.item() - want['pg']),
                   pg_rel=abs(got.extra.policy_gradient_loss.item() - want['pg']) / max(abs(want['pg']), 1e-30))
