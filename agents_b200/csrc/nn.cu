@@ -508,6 +508,7 @@ __global__ void __launch_bounds__(256) skinny_dx_kernel(const float* __restrict_
   __syncthreads();
   const int kq = (K + 3) >> 2;                        // k quads per row
   const int64_t total = M * kq;
+  const bool vec = (K & 3) == 0 && ((uintptr_t)dX & 15) == 0;   // dX is a caller pointer
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t m = i / kq;
@@ -527,7 +528,7 @@ __global__ void __launch_bounds__(256) skinny_dx_kernel(const float* __restrict_
       }
     }
     float* dst = dX + m * K + k0;
-    if ((K & 3) == 0) *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1], o[2], o[3]);
+    if (vec) *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1], o[2], o[3]);
     else
       for (int q = 0; q < 4; ++q)
         if (k0 + q < K) dst[q] = o[q];
@@ -882,14 +883,17 @@ static int gemm_mode() {
 template <int BN, int PASSES, int EPI, class AL, class BL>
 static int launch_tc_cfg(const AL& a, const BL& b, const GemmArgs& g, const tc::EpiArgs& epi) {
   using L = tc::SmemLayout<BN, PASSES, AL::kExact>;
-  auto kernel = tc::tc_gemm_kernel<BN, PASSES, EPI, AL, BL>;
+  auto short_k = tc::tc_gemm_kernel<BN, PASSES, EPI, AL, BL, false>;
+  auto long_k = tc::tc_gemm_kernel<BN, PASSES, EPI, AL, BL, PASSES == 3>;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         L::kBytes);
-    if (e != cudaSuccess) {
-      set_error("tc_gemm: cannot set dynamic smem to %d: %s", L::kBytes, cudaGetErrorString(e));
-      return B200RL_ERR_CUDA;
+    for (auto kernel : {short_k, long_k}) {
+      cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           L::kBytes);
+      if (e != cudaSuccess) {
+        set_error("tc_gemm: cannot set dynamic smem to %d: %s", L::kBytes, cudaGetErrorString(e));
+        return B200RL_ERR_CUDA;
+      }
     }
     configured = true;
   }
@@ -912,6 +916,8 @@ static int launch_tc_cfg(const AL& a, const BL& b, const GemmArgs& g, const tc::
   if (splits < 1) splits = 1;
   B200RL_CHECK_ARG(tm <= 65535, "tc_gemm: M too large for grid.y (%lld tiles)", (long long)tm);
   dim3 grid((unsigned)tn, (unsigned)tm, (unsigned)splits);
+  // a K range longer than one accumulation chain needs the chained variant to stay fp32-accurate
+  auto kernel = kps > tc::kChainBlocks * tc::kBK ? long_k : short_k;
   B200RL_LAUNCH(kernel, grid, tc::kThreads, L::kBytes, g.st, a, b, epi, g.C, g.bias, g.M, g.N, g.K, g.act, g.beta, splits, kps, (float*)g.ws, g.out_scale);
   B200RL_CHECK_LAUNCH("tc_gemm");
   if (splits > 1 && EPI == tc::EPI_STORE) {

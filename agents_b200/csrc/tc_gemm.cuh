@@ -32,6 +32,7 @@ constexpr int kBM = 128;
 constexpr int kBK = 32;                    // fp32 elements = 128 bytes = one swizzle row
 constexpr int kThreads = 256;
 constexpr int kStages = 3;
+constexpr int kChainBlocks = 8;           // K blocks per tensor-core accumulation chain (CHAINS)
 
 // optional phase stamps (b200rl_tc_debug_buffer): [block][8] nanosecond timers
 __device__ long long* g_tc_dbg = nullptr;
@@ -61,20 +62,21 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   return d;
 }
 
-// D[64 x N] += A[64 x 8] * B[8 x N], both operands from shared memory (descriptors above).
+// D[64 x N] = A[64 x 8] * B[8 x N] + (scale_d ? D : 0), both operands from shared memory
+// (descriptors above).
 template <int N>
-__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t a, uint64_t b);
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t a, uint64_t b, int scale_d);
 template <>
-__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t a, uint64_t b, int scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(a), "l"(b), "r"(1));
+      : "l"(a), "l"(b), "r"(scale_d));
 }
 template <>
-__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t a, uint64_t b, int scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
@@ -82,10 +84,10 @@ __device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t a, uint6
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
         "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
         "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(a), "l"(b), "r"(1));
+      : "l"(a), "l"(b), "r"(scale_d));
 }
 template <>
-__device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t a, uint64_t b, int scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}"
@@ -97,7 +99,7 @@ __device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t a, uint
         "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
         "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
         "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(a), "l"(b), "r"(1));
+      : "l"(a), "l"(b), "r"(scale_d));
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -259,9 +261,10 @@ __device__ __forceinline__ void scatter_tile_mn(unsigned char* hi, unsigned char
 // Epilogue variants.  EPI_STORE: C (+)= act(acc + bias) or split-K partial.  EPI_COL2IM: the
 // GEMM is dcol[pos, (ky,kx,c)] = dY @ W^T of a convolution input gradient and every 4-channel
 // group is scatter-added straight into dX[n, oy*s+ky, ox*s+kx, c..c+3] with one
-// red.global.add.v4.f32 — the [M, KH*KW*C] dcol matrix is never materialised and split-K
-// partials need no reduction pass (dX must be zeroed by the caller; summation order of the
-// <= KH*KW/s^2 contributions per element is not fixed).
+// red.global.add.v4.f32 (four scalar atomics when dX is not 16-byte aligned) — the
+// [M, KH*KW*C] dcol matrix is never materialised and split-K partials need no reduction pass
+// (dX must be zeroed by the caller; summation order of the <= KH*KW/s^2 contributions per
+// element is not fixed).
 constexpr int EPI_STORE = 0;
 constexpr int EPI_COL2IM = 1;
 constexpr int EPI_ATOMIC = 2;  // C += acc with red.global.add (split-K without a reduce pass; C pre-zeroed)
@@ -273,7 +276,8 @@ struct EpiArgs {
 };
 
 // AL / BL are the fp32 operand views of nn.cu (row index = m for A, n for B).
-template <int BN, int PASSES, int EPI, class AL, class BL>
+// CHAINS: the K range of a CTA is long (> kChainBlocks blocks), see `sum` below.
+template <int BN, int PASSES, int EPI, class AL, class BL, bool CHAINS>
 __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const BL b,
                                                               const EpiArgs epi,
                                                               float* __restrict__ C,
@@ -346,9 +350,17 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const 
   const bool do_colsum = EPI == EPI_ATOMIC && !BL::kKContig && epi.colsum != nullptr &&
                          blockIdx.y == 0;
   float4 bsum = make_float4(0.f, 0.f, 0.f, 0.f);
-  float acc[BN / 2];
+  // The wgmma accumulator does not round to nearest: every accumulate loses ~2^-24 of the running
+  // sum, always toward zero, so on same-sign data one chain over K = 3136 drifts by ~7e-5 (512:
+  // 1.2e-5, 256: 6.6e-6).  With CHAINS, each chain covers kChainBlocks K blocks only and is then
+  // added into `sum` with an ordinary (round-to-nearest) fp32 add; the next chain restarts the
+  // accumulator (scale-d = 0).  `sum` costs BN/2 registers, which slows the BN=128 kernels by ~12 %
+  // even when no chain ends, so the host selects CHAINS only for K ranges longer than one chain.
+  float acc[BN / 2], sum[CHAINS ? BN / 2 : 1];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < (CHAINS ? BN / 2 : 1); ++i) sum[i] = 0.f;
   if (nkb > 0) {
     gather_a(kb, av);
     gather_b(kb, bv);
@@ -385,19 +397,29 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const 
     const uint32_t sa = smem_base + (uint32_t)s * L::kStage + (uint32_t)wg * (64u * 128u);
     const uint32_t sb = smem_base + (uint32_t)s * L::kStage + L::kNumA * L::kATile;
     const uint32_t a_lo_off = L::kATile, b_lo_off = L::kBTile;
+    const bool fresh = CHAINS && kbi % kChainBlocks == 0;   // first block of a chain
+    if constexpr (CHAINS) {
+      if (fresh && kbi > 0) {
+        // the previous block's MMAs ran during this block's gather/scatter; usually retired
+        wgmma_wait<0>();
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) sum[i] += acc[i];
+      }
+    }
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < kBK / 8; ++ks) {
       const uint32_t ko = (uint32_t)ks * 32u;   // 8 tf32 = 32 bytes further inside the 128 B row
+      const int keep = (fresh && ks == 0) ? 0 : 1;   // scale-d of the block's first MMA
       if (PASSES == 3 && AL::kExact) {
-        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + b_lo_off + ko));
-        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko));
+        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + b_lo_off + ko), keep);
+        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko), 1);
       } else if (PASSES == 3) {
-        wgmma_tf32<BN>(acc, make_desc(sa + a_lo_off + ko), make_desc(sb + ko));
-        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + b_lo_off + ko));
-        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko));
+        wgmma_tf32<BN>(acc, make_desc(sa + a_lo_off + ko), make_desc(sb + ko), keep);
+        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + b_lo_off + ko), 1);
+        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko), 1);
       } else {
-        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko));
+        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko), keep);
       }
     }
     wgmma_commit();
@@ -409,6 +431,10 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const 
     if (kbi + 1 < nkb) k_block(kbi + 1, an, bn, av, bv);
   }
   wgmma_wait<0>();
+  if constexpr (CHAINS) {
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] += sum[i];   // the last chain (all zero when nkb == 0)
+  }
   if (tid == 0) stamp(2);
   __syncthreads();   // every MMA of the CTA has retired: the stage buffers hold the staging tile now
 
@@ -469,6 +495,10 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const 
       // act'(X) of the layer that produced the conv input: the scatter-add is linear, so every
       // contribution is masked on its way out (X is read at the destination index)
       const float* ybase = epi.mask.y ? epi.mask.y + (int64_t)img * epi.mask.ld + in_off : nullptr;
+      // C % 4 == 0 keeps every 4-channel group 16-byte aligned relative to dX / X; the base
+      // pointers (and the X image stride) are the caller's and need not be
+      const bool dx_vec = ((uintptr_t)epi.dx & 15) == 0;
+      const bool y_vec = ((uintptr_t)epi.mask.y & 15) == 0 && (epi.mask.ld & 3) == 0;
 #pragma unroll
       for (int j = 0; j < G; j += 4) {
         const int64_t kidx = nb + j;
@@ -478,20 +508,27 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const 
         float* dst = base + (int64_t)ky * wc + rr;
         float4 v = make_float4(r[j], r[j + 1], r[j + 2], r[j + 3]);
         if (ybase) {
-          const float4 y = *reinterpret_cast<const float4*>(ybase + (int64_t)ky * wc + rr);
+          const float* yp = ybase + (int64_t)ky * wc + rr;
+          const float4 y = y_vec ? *reinterpret_cast<const float4*>(yp)
+                                 : make_float4(yp[0], yp[1], yp[2], yp[3]);
           v.x = dact(y.x, v.x, epi.mask.act); v.y = dact(y.y, v.y, epi.mask.act);
           v.z = dact(y.z, v.z, epi.mask.act); v.w = dact(y.w, v.w, epi.mask.act);
         }
-        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x),
-                     "f"(v.y), "f"(v.z), "f"(v.w)
-                     : "memory");
+        if (dx_vec) {
+          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x),
+                       "f"(v.y), "f"(v.z), "f"(v.w)
+                       : "memory");
+        } else {
+          atomicAdd(dst + 0, v.x); atomicAdd(dst + 1, v.y);
+          atomicAdd(dst + 2, v.z); atomicAdd(dst + 3, v.w);
+        }
       }
       continue;
     }
     if (EPI == EPI_ATOMIC) {
       if (nkb == 0) continue;
       float* dst = C + m * N + nb;
-      if ((N & 3) == 0 && nb + G - 1 < N) {
+      if ((N & 3) == 0 && ((uintptr_t)C & 15) == 0 && nb + G - 1 < N) {
 #pragma unroll
         for (int j = 0; j < G; j += 4)
           asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j),

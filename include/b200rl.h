@@ -357,10 +357,11 @@ int b200rl_dense_fwd(const float* X, int64_t ldx, const float* W, const float* b
                      int64_t M, int64_t K, int64_t N, int act, void* workspace,
                      int64_t ws_bytes, void* stream);
 /* Two dense layers of identical shape (X1 @ W1 + b1 -> Y1, X2 @ W2 + b2 -> Y2; biases both given
- * or both NULL) in ONE launch of the persistent tensor-core kernel; two launches when that kernel
- * does not take the shape.  DqnAgent evaluates the online network on obs[:, 0] and the target
- * network on obs[:, T-1] this way (agents/dqn/dqn_agent.py:488-520, :575-579 in the reference are
- * the two independent forward passes).  Workspace as b200rl_dense_fwd (split-K needs room for both). */
+ * or both NULL) in one call: the same GEMM route as b200rl_dense_fwd, launched once per layer
+ * (two launches, plus a split-K reduce each when the shape splits).  DqnAgent evaluates the
+ * online network on obs[:, 0] and the target network on obs[:, T-1] this way
+ * (agents/dqn/dqn_agent.py:488-520, :575-579 in the reference are the two independent forward
+ * passes).  Workspace as b200rl_dense_fwd; the two launches use it one after the other. */
 int b200rl_dense_fwd_pair(const float* X1, const float* X2, int64_t ldx, const float* W1,
                           const float* W2, const float* bias1, const float* bias2, float* Y1,
                           float* Y2, int64_t M, int64_t K, int64_t N, int act, void* workspace,
@@ -391,7 +392,8 @@ typedef struct {
 int b200rl_conv2d_fwd(const void* X, int x_is_u8, float x_scale, const float* Wt,
                       const float* bias, float* Y, const b200rl_conv_t* g, int act,
                       void* workspace, int64_t ws_bytes, void* stream);
-/* Two convolutions of identical geometry in one launch (see b200rl_dense_fwd_pair). */
+/* Two convolutions of identical geometry in one call, launched once per convolution (see
+ * b200rl_dense_fwd_pair). */
 int b200rl_conv2d_fwd_pair(const void* X1, const void* X2, int x_is_u8, float x_scale,
                            const float* Wt1, const float* Wt2, const float* bias1,
                            const float* bias2, float* Y1, float* Y2, const b200rl_conv_t* c,
