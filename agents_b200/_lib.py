@@ -50,6 +50,11 @@ class PpoKl(ctypes.Structure):
               ('terms', c_void_p), ('grad_scale', c_f32)]
 
 
+class PpoKlLogits(ctypes.Structure):
+  _fields_ = [('old_logits', c_void_p), ('ld_old', c_i64), ('terms', c_void_p),
+              ('grad_scale', c_f32)]
+
+
 class B200RLError(RuntimeError):
   pass
 
@@ -80,6 +85,13 @@ SIGNATURES = {
     'b200rl_ppo_kl_beta_update': [_P, _P, c_f32, c_f32, _P],
     'b200rl_normal_logp': [_P, _P, c_i64, _P, c_i64, c_i64, _P, _P],
     'b200rl_normal_sample': [_P, _P, c_i64, c_i64, c_i64, _P, _P, c_u64, _P, _P, _P],
+    'b200rl_ppo_loss_categorical': [_P, c_i64, _P, _P, _P, _P, _P, _P, _P, c_i64, c_i64, c_i64,
+                                    c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, _P, _P, c_i64, _P,
+                                    _P, _P, _P, c_i64, _P],
+    'b200rl_categorical_logp': [_P, c_i64, _P, c_i64, c_i64, _P, _P, _P],
+    'b200rl_ppo_kl_categorical': [_P, c_i64, _P, c_i64, _P, c_i64, c_i64, c_f32, _P, _P, _P,
+                                  c_i64, _P],
+    'b200rl_categorical_sample': [_P, c_i64, c_i64, c_i64, c_u64, _P, _P, _P],
     'b200rl_normal_proj_fwd': [_P, _P, _P, _P, c_i64, c_i64, _P, _P, _P],
     'b200rl_normal_proj_bwd': [_P, _P, _P, _P, _P, _P, c_i64, c_i64, _P, _P, _P],
     'b200rl_colsum': [_P, _P, c_int, c_i64, c_i64, c_f32, _P, _P, c_i64, _P],

@@ -8,6 +8,9 @@ updates per `train` call with global-norm clipping and ONE optimiser over actor 
 parameters, and the KL penalty of the original formulation (ppo_agent.py:1514-1690): squared
 KL-cutoff loss + adaptive-beta loss inside every epoch, beta updated once after the epochs.
 PPOClipAgent sets both to zero (ppo_clip_agent.py:226-232) and skips that work entirely.
+The policy is a diagonal Normal for a continuous action spec and a Categorical over logits for a
+discrete one (ppo_agent.py:48, actor_distribution_network.py:157-158); `_train` is shared and only
+the behaviour log-probs, the loss launch, the KL and the actor backward follow the distribution.
 
 Device work of `train(experience[B, T])` (csrc/ppo.cu, scans.cu, nn.cu, optim.cu):
   value net on B*T observations -> gamma*d*episode_mask -> returns scan -> GAE scan (warp-shuffle
@@ -212,13 +215,21 @@ class PPOAgent(tf_agent.TFAgent):
       weights = torch.as_tensor(weights, dtype=torch.float32, device=dev).expand(B, T).contiguous()
     _lib.call('b200rl_ppo_weights', _lib.ptr(experience.step_type.to(torch.int32).contiguous()),
               _lib.ptr(returns), _lib.ptr(adv), _lib.ptr(weights), N, _lib.ptr(w), st)
-    action = experience.action.float().reshape(N, A).contiguous()
+    discrete = self._actor_net.discrete
     old = experience.policy_info['dist_params']
-    old_loc = old['loc'].float().reshape(N, A).contiguous()
-    old_scale = old['scale'].float().reshape(N, A).contiguous()
     old_logp = torch.empty(N, dtype=torch.float32, device=dev)
-    _lib.call('b200rl_normal_logp', _lib.ptr(old_loc), _lib.ptr(old_scale), A, _lib.ptr(action), N,
-              A, _lib.ptr(old_logp), st)
+    if discrete:                                                  # integer actions read as int32
+      action = experience.action.reshape(N).to(torch.int32).contiguous()
+      old_params = old['logits'].float().reshape(N, A).contiguous()
+      _lib.call('b200rl_categorical_logp', _lib.ptr(old_params), A, _lib.ptr(action), N, A,
+                _lib.ptr(old_logp), _lib.ptr(self._nan_flag), st)
+    else:
+      action = experience.action.float().reshape(N, A).contiguous()
+      old_loc = old['loc'].float().reshape(N, A).contiguous()
+      old_scale = old['scale'].float().reshape(N, A).contiguous()
+      old_params = (old_loc, old_scale)
+      _lib.call('b200rl_normal_logp', _lib.ptr(old_loc), _lib.ptr(old_scale), A, _lib.ptr(action),
+                N, A, _lib.ptr(old_logp), st)
     # _normalize_advantages over axes (0, 1), unmasked (:893-895, :100-110); sharded runs merge
     # the per-rank moments with one collective (tensor_normalizer.batch_moments)
     mean = torch.empty(1, dtype=torch.float32, device=dev)
@@ -240,28 +251,43 @@ class PPOAgent(tf_agent.TFAgent):
       # mean_kl is the mean over the GLOBAL batch (per-rank partial sums are SUM-reduced) and the
       # KL gradient carries 1/N_global, so R replicas reproduce the one-device update on the
       # concatenated batch (the reference's per-replica reduce_mean would weigh the penalty R x).
-      kl_arg = _lib.PpoKl(_lib.ptr(old_loc), _lib.ptr(old_scale), A, _lib.ptr(self._kl_terms),
-                          1.0 / n_glob)
+      if discrete:
+        kl_arg = _lib.PpoKlLogits(_lib.ptr(old_params), A, _lib.ptr(self._kl_terms), 1.0 / n_glob)
+      else:
+        kl_arg = _lib.PpoKl(_lib.ptr(old_loc), _lib.ptr(old_scale), A, _lib.ptr(self._kl_terms),
+                            1.0 / n_glob)
     l2 = torch.zeros(1, dtype=torch.float32, device=dev)
-    dloc = torch.empty((N, A), dtype=torch.float32, device=dev)
-    dscale = torch.empty((N, A), dtype=torch.float32, device=dev)
+    if discrete:
+      dlogits = torch.empty((N, A), dtype=torch.float32, device=dev)
+    else:
+      dloc = torch.empty((N, A), dtype=torch.float32, device=dev)
+      dscale = torch.empty((N, A), dtype=torch.float32, device=dev)
     dv = torch.empty((N, 1), dtype=torch.float32, device=dev)
     gb = float(B * self.replicas)
+    scalars = (float(self._importance_ratio_clipping), float(self._value_clipping),
+               float(self._value_pred_loss_coef), float(self._entropy_regularization),
+               float(self._log_prob_clipping))
     for _ in range(self._num_epochs):                             # :925-967
-      (loc, scale), actx = self._actor_net.forward_train(obs_n)
+      params, actx = self._actor_net.forward_train(obs_n)
       v, vtape = self._value_net.forward_train(obs_n)
       if use_kl:
-        self._mean_kl(loc, scale, old_loc, old_scale, w, N, A, n_glob)
+        self._mean_kl(params, old_params, w, N, A, n_glob)
         self._kl_penalty_terms()
-      _lib.call('b200rl_ppo_loss', _lib.ptr(loc), _lib.ptr(scale), A, _lib.ptr(action),
-                _lib.ptr(old_logp), _lib.ptr(adv_n), _lib.ptr(returns), _lib.ptr(v), _lib.ptr(vp),
-                _lib.ptr(w), N, A, T, gb, float(self._importance_ratio_clipping),
-                float(self._value_clipping), float(self._value_pred_loss_coef),
-                float(self._entropy_regularization), float(self._log_prob_clipping),
-                _lib.ptr(losses), _lib.ptr(dloc), _lib.ptr(dscale), A, _lib.ptr(dv),
-                _lib.ptr(self._nan_flag), ctypes.byref(kl_arg) if use_kl else None, _lib.ptr(ws),
-                nb, st)
-      self._actor_net.backward(actx, (dloc, dscale))
+      if discrete:
+        _lib.call('b200rl_ppo_loss_categorical', _lib.ptr(params), A, _lib.ptr(action),
+                  _lib.ptr(old_logp), _lib.ptr(adv_n), _lib.ptr(returns), _lib.ptr(v),
+                  _lib.ptr(vp), _lib.ptr(w), N, A, T, gb, *scalars, _lib.ptr(losses),
+                  _lib.ptr(dlogits), A, _lib.ptr(dv), _lib.ptr(self._nan_flag),
+                  ctypes.byref(kl_arg) if use_kl else None, _lib.ptr(ws), nb, st)
+        self._actor_net.backward(actx, dlogits)
+      else:
+        loc, scale = params
+        _lib.call('b200rl_ppo_loss', _lib.ptr(loc), _lib.ptr(scale), A, _lib.ptr(action),
+                  _lib.ptr(old_logp), _lib.ptr(adv_n), _lib.ptr(returns), _lib.ptr(v),
+                  _lib.ptr(vp), _lib.ptr(w), N, A, T, gb, *scalars, _lib.ptr(losses),
+                  _lib.ptr(dloc), _lib.ptr(dscale), A, _lib.ptr(dv), _lib.ptr(self._nan_flag),
+                  ctypes.byref(kl_arg) if use_kl else None, _lib.ptr(ws), nb, st)
+        self._actor_net.backward(actx, (dloc, dscale))
       self._value_net.backward(vtape, dv)
       l2.zero_()
       self._l2_regularization(l2)
@@ -276,8 +302,8 @@ class PPOAgent(tf_agent.TFAgent):
       self._optimizer.apply_flat(self._flat_params, self._flat_grads, scale_dev)
       self._bump_train_step(1)
     if self._initial_adaptive_kl_beta > 0:                        # :978-989
-      loc, scale = self._actor_net.distribution_params(obs_n)
-      self._mean_kl(loc, scale, old_loc, old_scale, w, N, A, n_glob)
+      params = self._actor_net.distribution_params(obs_n)
+      self._mean_kl(params, old_params, w, N, A, n_glob)
       self._update_beta()
     if self.update_normalizers_in_train:                          # :991-993
       self.update_observation_normalizer(obs)
@@ -290,12 +316,20 @@ class PPOAgent(tf_agent.TFAgent):
     return tf_agent.LossInfo(losses[4] + l2.reshape(()), extra)
 
   # ---- KL penalty (ppo_agent.py:1514-1690) ------------------------------------------------------
-  def _mean_kl(self, loc, scale, old_loc, old_scale, w, N, A, n_glob, out_kl=None):
-    """self._kl_mean <- sum_n w_n KL(old_n || new_n) / N_global (all-reduced when sharded)."""
-    ws, nb = workspace.get(loc.device)
-    _lib.call('b200rl_ppo_kl', _lib.ptr(loc), _lib.ptr(scale), A, _lib.ptr(old_loc),
-              _lib.ptr(old_scale), A, _lib.ptr(w), N, A, 1.0 / n_glob, _lib.ptr(out_kl),
-              _lib.ptr(self._kl_mean), _lib.ptr(ws), nb, _lib.stream())
+  def _mean_kl(self, params, old_params, w, N, A, n_glob, out_kl=None):
+    """self._kl_mean <- sum_n w_n KL(old_n || new_n) / N_global (all-reduced when sharded).
+    params / old_params: [N, A] logits (Categorical) or (loc, scale) pairs (Normal)."""
+    if self._actor_net.discrete:
+      ws, nb = workspace.get(params.device)
+      _lib.call('b200rl_ppo_kl_categorical', _lib.ptr(params), A, _lib.ptr(old_params), A,
+                _lib.ptr(w), N, A, 1.0 / n_glob, _lib.ptr(out_kl), _lib.ptr(self._kl_mean),
+                _lib.ptr(ws), nb, _lib.stream())
+    else:
+      (loc, scale), (old_loc, old_scale) = params, old_params
+      ws, nb = workspace.get(loc.device)
+      _lib.call('b200rl_ppo_kl', _lib.ptr(loc), _lib.ptr(scale), A, _lib.ptr(old_loc),
+                _lib.ptr(old_scale), A, _lib.ptr(w), N, A, 1.0 / n_glob, _lib.ptr(out_kl),
+                _lib.ptr(self._kl_mean), _lib.ptr(ws), nb, _lib.stream())
     if self._stat_sync is not None:
       self._stat_sync(self._kl_mean)
 
@@ -340,17 +374,21 @@ class PPOAgent(tf_agent.TFAgent):
   def kl_penalty_loss(self, time_steps, action_distribution_parameters,
                       current_policy_distribution, weights, debug_summaries=False):
     """kl_cutoff_loss + adaptive_kl_loss of weights * KL(old || current) (:1586-1630).
-    `current_policy_distribution` is a (loc, scale) pair of [N, A] tensors."""
-    loc, scale = current_policy_distribution
-    old_loc = action_distribution_parameters['loc'].float()
-    old_scale = action_distribution_parameters['scale'].float()
-    A = loc.shape[-1]
-    loc, scale = loc.reshape(-1, A).contiguous(), scale.reshape(-1, A).contiguous()
-    old_loc, old_scale = old_loc.reshape(-1, A).contiguous(), old_scale.reshape(-1, A).contiguous()
-    N = loc.shape[0]
-    w = torch.as_tensor(weights, dtype=torch.float32, device=loc.device).reshape(-1).contiguous()
-    kl = torch.empty(N, dtype=torch.float32, device=loc.device)
-    self._mean_kl(loc, scale, old_loc, old_scale, w, N, A, float(N * self.replicas), out_kl=kl)
+    `current_policy_distribution` is a (loc, scale) pair of [N, A] tensors, or the [N, A] logits
+    for a discrete action (then `action_distribution_parameters` holds 'logits')."""
+    flat = lambda t: t.float().reshape(-1, t.shape[-1]).contiguous()
+    if self._actor_net.discrete:
+      params = flat(current_policy_distribution)
+      old_params = flat(action_distribution_parameters['logits'])
+      dev, (N, A) = params.device, params.shape
+    else:
+      params = tuple(flat(t) for t in current_policy_distribution)
+      old_params = (flat(action_distribution_parameters['loc']),
+                    flat(action_distribution_parameters['scale']))
+      dev, (N, A) = params[0].device, params[0].shape
+    w = torch.as_tensor(weights, dtype=torch.float32, device=dev).reshape(-1).contiguous()
+    kl = torch.empty(N, dtype=torch.float32, device=dev)
+    self._mean_kl(params, old_params, w, N, A, float(N * self.replicas), out_kl=kl)
     # through the public methods, like the reference (its test mocks them)
     return self.kl_cutoff_loss(kl, debug_summaries) + self.adaptive_kl_loss(kl, debug_summaries)
 

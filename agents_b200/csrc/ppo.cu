@@ -403,6 +403,258 @@ __global__ void ppo_kl_beta_update_kernel(const float* __restrict__ mean_kl,
   *beta = fminf(fmaxf(*beta * f, 10e-16f), 10e16f);
 }
 
+// ---- Categorical policy (discrete actions): CategoricalProjectionNetwork logits [N, A] --------
+// A row of logits is handled by a group of G lanes (lane l takes columns l, l+G, ...); G follows
+// from A (cat_group): one thread per row for narrow rows, 8 or 32 lanes with shuffle reductions
+// for wide ones, so a row is read with coalesced loads.  Every warp runs the same number of row
+// iterations (groups past N repeat their warp's first row and discard the result), so the
+// full-mask shuffles never diverge.
+template <int G>
+__device__ __forceinline__ float grp_max(float v) {
+#pragma unroll
+  for (int o = G / 2; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o, G));
+  return v;
+}
+template <int G>
+__device__ __forceinline__ float grp_sum(float v) {
+#pragma unroll
+  for (int o = G / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o, G);
+  return v;
+}
+
+// Max-subtracted log-softmax statistics of one row: m = max z, s = sum exp(z - m),
+// t = sum exp(z - m) * (z - m).  log p_j = (z_j - m) - log s, entropy = log s - t / s.
+template <int G>
+__device__ __forceinline__ void row_softmax_stats(const float* __restrict__ z, int64_t A, int lane,
+                                                  float& m, float& s, float& t) {
+  m = -INFINITY;
+  for (int64_t j = lane; j < A; j += G) m = fmaxf(m, z[j]);
+  m = grp_max<G>(m);
+  s = 0.f; t = 0.f;
+  for (int64_t j = lane; j < A; j += G) {
+    const float d = z[j] - m;
+    const float e = expf(d);
+    s += e;
+    t += e > 0.f ? e * d : 0.f;
+  }
+  s = grp_sum<G>(s);
+  t = grp_sum<G>(t);
+}
+
+// Row iteration shared by the group kernels: n is this group's row, n0 the row of the warp's first
+// group (warp-uniform loop bound).
+#define B200RL_GROUP_ROWS(G, N)                                                              \
+  const int lane = (int)(threadIdx.x % (G));                                                 \
+  const int64_t stride_ = (int64_t)gridDim.x * blockDim.x / (G);                             \
+  for (int64_t n = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / (G),                   \
+               n0 = ((int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) / (G);         \
+       n0 < (N); n += stride_, n0 += stride_)
+
+__device__ __forceinline__ int clamp_action(int32_t a, int64_t A, int32_t* nan_flag) {
+  if (a < 0 || a >= A) {          // out-of-range action: read a valid column, report it
+    if (nan_flag) *nan_flag = 1;
+    a = a < 0 ? 0 : (int32_t)(A - 1);
+  }
+  return a;
+}
+
+struct PpoCatArgs {
+  const float* logits; int64_t ld;                           // current policy Categorical(logits)
+  const int32_t* action;                                     // [N]
+  const float* old_logp; const float* adv; const float* ret; // [N]
+  const float* v; const float* v_old; const float* w;        // [N]
+  int64_t N, A, T;
+  float global_batch, clip_eps, value_clip, vf_coef, ent_coef, logp_clip;
+  float* dlogits; int64_t ld_g;
+  float* dv;
+  float* partial;                                            // [kCatRedBlocks, 4]
+  int32_t* nan_flag;
+  // KL penalty: behaviour policy Categorical(old_logits); d(kl_penalty)/d(mean_kl) in kl_terms[2]
+  const float* old_logits; int64_t ld_old;
+  const float* kl_terms; float kl_grad_scale;
+};
+
+// The categorical twin of ppo_loss_kernel: same surrogate / value / entropy terms and the same
+// 4-partial layout for ppo_loss_final_kernel.  dL/dz_j = g_logp (1[j=a] - p_j)
+// + g_ent (-p_j (log p_j + H)) + g_kl (p_j - q_j), q = softmax(old_logits).
+template <int G>
+__global__ void __launch_bounds__(256) ppo_loss_cat_kernel(const PpoCatArgs a) {
+  pdl_prologue();
+  __shared__ float red[32];
+  float s_pg = 0.f, s_ve = 0.f, s_ent = 0.f, s_clip = 0.f;
+  const float denom = (float)a.T * a.global_batch;
+  B200RL_GROUP_ROWS(G, a.N) {
+    const bool valid = n < a.N;
+    const int64_t r = valid ? n : n0;
+    const float* z = a.logits + r * a.ld;
+    const int act = clamp_action(a.action[r], a.A, valid ? a.nan_flag : nullptr);
+    float m, s, t;
+    row_softmax_stats<G>(z, a.A, lane, m, s, t);
+    const float log_s = logf(s);
+    const float ent = log_s - t / s;
+    const float logp = (z[act] - m) - log_s;
+    float lp = logp, dlp = 1.f;
+    if (a.logp_clip > 0.f) {
+      lp = fminf(fmaxf(logp, -a.logp_clip), a.logp_clip);
+      dlp = (logp < -a.logp_clip || logp > a.logp_clip) ? 0.f : 1.f;
+    }
+    const float w = a.w[r];
+    const float A_hat = a.adv[r];
+    const float ratio = expf(lp - a.old_logp[r]);
+    const float lo = 1.f - a.clip_eps, hi = 1.f + a.clip_eps;
+    const float ratio_c = fminf(fmaxf(ratio, lo), hi);
+    const float obj = ratio * A_hat, obj_c = ratio_c * A_hat;
+    float pg, dobj_dratio, clipped = 0.f;
+    if (a.clip_eps > 0.f) {
+      pg = -fminf(obj, obj_c);
+      if (obj <= obj_c) dobj_dratio = A_hat;
+      else dobj_dratio = (ratio < lo || ratio > hi) ? 0.f : A_hat;
+      clipped = (fabsf(ratio - 1.f) > a.clip_eps) ? 1.f : 0.f;
+    } else {
+      pg = -obj;
+      dobj_dratio = A_hat;
+    }
+    const float R = a.ret[r], v = a.v[r];
+    float err = (R - v) * (R - v);
+    float derr_dv = -2.f * (R - v);
+    if (a.value_clip > 0.f) {
+      const float vo = a.v_old[r];
+      const float dvv = v - vo;
+      const float vc = vo + fminf(fmaxf(dvv, -a.value_clip), a.value_clip);
+      const float err_c = (R - vc) * (R - vc);
+      if (err_c > err) {
+        err = err_c;
+        derr_dv = (dvv < -a.value_clip || dvv > a.value_clip) ? 0.f : -2.f * (R - vc);
+      }
+    }
+    if (valid && lane == 0) {
+      s_pg += pg * w;
+      s_ve += err * w;
+      s_ent += -ent * w;
+      s_clip += clipped;
+      a.dv[r] = a.vf_coef * derr_dv * w / denom;
+    }
+    const float g_logp = -dobj_dratio * ratio * dlp * w / denom;
+    const float g_ent = -a.ent_coef * w / denom;
+    float g_kl = 0.f, mo = 0.f, lso = 0.f;
+    const float* zo = nullptr;
+    if (a.kl_terms) {
+      g_kl = a.kl_terms[2] * a.kl_grad_scale * w;
+      zo = a.old_logits + r * a.ld_old;
+      float so, to;
+      row_softmax_stats<G>(zo, a.A, lane, mo, so, to);
+      lso = logf(so);
+    }
+    if (valid) {
+      for (int64_t j = lane; j < a.A; j += G) {
+        const float lpj = (z[j] - m) - log_s;
+        const float p = expf(lpj);
+        float g = g_logp * ((j == act ? 1.f : 0.f) - p) + g_ent * (-p * (lpj + ent));
+        if (zo) g += g_kl * (p - expf((zo[j] - mo) - lso));
+        a.dlogits[r * a.ld_g + j] = g;
+      }
+    }
+  }
+  const float t_pg = block_sum(s_pg, red);
+  const float t_ve = block_sum(s_ve, red);
+  const float t_ent = block_sum(s_ent, red);
+  const float t_clip = block_sum(s_clip, red);
+  if (threadIdx.x == 0) {
+    float* p = a.partial + (int64_t)blockIdx.x * 4;
+    p[0] = t_pg; p[1] = t_ve; p[2] = t_ent; p[3] = t_clip;
+  }
+}
+
+template <int G>
+__global__ void __launch_bounds__(256) categorical_logp_kernel(const float* __restrict__ logits,
+                                                               int64_t ld,
+                                                               const int32_t* __restrict__ action,
+                                                               int64_t N, int64_t A,
+                                                               float* __restrict__ out,
+                                                               int32_t* nan_flag) {
+  pdl_prologue();
+  B200RL_GROUP_ROWS(G, N) {
+    const bool valid = n < N;
+    const int64_t r = valid ? n : n0;
+    const float* z = logits + r * ld;
+    const int act = clamp_action(action[r], A, valid ? nan_flag : nullptr);
+    float m, s, t;
+    row_softmax_stats<G>(z, A, lane, m, s, t);
+    if (valid && lane == 0) out[r] = (z[act] - m) - logf(s);
+  }
+}
+
+// sum_n w_n * KL(Categorical(old)_n || Categorical(new)_n), KL = sum_j q_j (log q_j - log p_j)
+// (tfp _kl_categorical_categorical), two fixed-order stages like ppo_kl_partial_kernel.
+template <int G>
+__global__ void __launch_bounds__(256) ppo_kl_cat_partial_kernel(
+    const float* __restrict__ logits, int64_t ld, const float* __restrict__ old_logits,
+    int64_t ld_old, const float* __restrict__ w, int64_t N, int64_t A, float* __restrict__ out_kl,
+    float* __restrict__ partial) {
+  pdl_prologue();
+  __shared__ float red[32];
+  float acc = 0.f;
+  B200RL_GROUP_ROWS(G, N) {
+    const bool valid = n < N;
+    const int64_t r = valid ? n : n0;
+    const float* z = logits + r * ld;
+    const float* zo = old_logits + r * ld_old;
+    float m, s, t, mo, so, to;
+    row_softmax_stats<G>(z, A, lane, m, s, t);
+    row_softmax_stats<G>(zo, A, lane, mo, so, to);
+    const float ls = logf(s), lso = logf(so);
+    float kl = 0.f;
+    for (int64_t j = lane; j < A; j += G) {
+      const float lq = (zo[j] - mo) - lso;
+      const float q = expf(lq);
+      kl += q > 0.f ? q * (lq - ((z[j] - m) - ls)) : 0.f;
+    }
+    kl = grp_sum<G>(kl);
+    kl *= w ? w[r] : 1.f;
+    if (valid && lane == 0) {
+      if (out_kl) out_kl[r] = kl;
+      acc += kl;
+    }
+  }
+  acc = block_sum(acc, red);
+  if (threadIdx.x == 0) partial[blockIdx.x] = acc;
+}
+
+// Collect-policy draw, one thread per row: u = uniform_f32(philox(counter=(n, call), key=seed).x);
+// action = smallest k with u < cdf_k, cdf the fp32 running sum in index order of
+// exp(z - max) / sum exp(z - max); A-1 if there is none.  rng_call: uint64[2] {call, ticket}.
+__global__ void categorical_sample_kernel(const float* __restrict__ logits, int64_t ld, int64_t N,
+                                          int64_t A, uint64_t seed, uint64_t* rng_call,
+                                          int32_t* __restrict__ out) {
+  pdl_prologue();
+  const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n < N) {
+    const float* z = logits + n * ld;
+    float m = z[0];
+    for (int64_t k = 1; k < A; ++k) m = fmaxf(m, z[k]);
+    float s = 0.f;
+    for (int64_t k = 0; k < A; ++k) s += expf(z[k] - m);
+    const float u = uniform_f32(philox4x32_10((uint64_t)n, rng_call[0], seed).x);
+    int32_t pick = (int32_t)(A - 1);
+    float cdf = 0.f;
+    for (int64_t k = 0; k < A; ++k) {
+      cdf += expf(z[k] - m) / s;
+      if (u < cdf) { pick = (int32_t)k; break; }
+    }
+    out[n] = pick;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    unsigned int tk = atomicAdd((uint32_t*)(rng_call + 1), 1u);
+    if (tk == gridDim.x - 1) {
+      *(uint32_t*)(rng_call + 1) = 0u;
+      rng_call[0] = rng_call[0] + 1;
+      __threadfence();
+    }
+  }
+}
+
 }  // namespace b200rl
 
 using namespace b200rl;
@@ -498,6 +750,105 @@ int b200rl_normal_sample(const float* loc, const float* scale, int64_t ld, int64
   B200RL_CHECK_ARG((amin == nullptr) == (amax == nullptr), "normal_sample: amin/amax mismatch");
   B200RL_LAUNCH(normal_sample_kernel, blocks_for(N * A), 256, 0, (cudaStream_t)stream, loc, scale, ld, N, A, amin, amax, seed, rng_call_dev, out);
   B200RL_CHECK_LAUNCH("normal_sample");
+  return B200RL_OK;
+}
+
+}  // extern "C"
+
+// Lanes per logits row: one thread for narrow rows, 8 or 32 lanes once a row spans more than
+// 8 / 64 columns (coalesced row reads, shuffle reductions).
+static int cat_group(int64_t A) { return A <= 8 ? 1 : (A <= 64 ? 8 : 32); }
+
+// The categorical kernels fill the GPU up to the 512 partials one 512-thread final kernel reduces
+// (about 4 CTAs of 256 per SM; the continuous kernels keep kRedBlocks).
+constexpr int kCatRedBlocks = 512;
+
+static unsigned cat_blocks(int64_t N, int G, int cap) {
+  int64_t nb = (N * G + 255) / 256;
+  return (unsigned)(nb > cap ? cap : nb);
+}
+
+extern "C" {
+
+int b200rl_ppo_loss_categorical(const float* logits, int64_t ld, const int32_t* action,
+                                const float* old_logp, const float* adv, const float* ret,
+                                const float* v, const float* v_old, const float* w, int64_t N,
+                                int64_t A, int64_t T, float global_batch, float clip_eps,
+                                float value_clip, float vf_coef, float ent_coef, float logp_clip,
+                                float* losses, float* dlogits, int64_t ld_g, float* dv,
+                                int32_t* nan_flag, const b200rl_ppo_kl_logits_t* kl,
+                                void* workspace, int64_t ws_bytes, void* stream) {
+  B200RL_CHECK_ARG(logits && action && old_logp && adv && ret && v && w && losses && dlogits && dv,
+                   "ppo_loss_categorical: NULL argument");
+  B200RL_CHECK_ARG(N >= 1 && A >= 1 && T >= 1 && global_batch > 0.f,
+                   "ppo_loss_categorical: bad sizes");
+  B200RL_CHECK_ARG(value_clip <= 0.f || v_old, "old_value_predictions is None but needed for value clipping.");
+  B200RL_CHECK_ARG(workspace && ws_bytes >= (int64_t)(kCatRedBlocks * 4 * sizeof(float)),
+                   "ppo_loss_categorical: workspace too small");
+  B200RL_CHECK_ARG(ld >= A && ld_g >= A, "ppo_loss_categorical: leading dimension < A");
+  cudaStream_t st = (cudaStream_t)stream;
+  PpoCatArgs a{logits, ld, action, old_logp, adv, ret, v, v_old, w, N, A, T, global_batch,
+               clip_eps, value_clip, vf_coef, ent_coef, logp_clip, dlogits, ld_g, dv,
+               (float*)workspace, nan_flag, nullptr, 0, nullptr, 0.f};
+  if (kl != nullptr) {
+    B200RL_CHECK_ARG(kl->old_logits && kl->terms && kl->ld_old >= A,
+                     "ppo_loss_categorical: incomplete KL-penalty arguments");
+    a.old_logits = kl->old_logits; a.ld_old = kl->ld_old;
+    a.kl_terms = kl->terms; a.kl_grad_scale = kl->grad_scale;
+  }
+  const int G = cat_group(A);
+  const unsigned nb = cat_blocks(N, G, kCatRedBlocks);
+  if (G == 1) B200RL_LAUNCH(ppo_loss_cat_kernel<1>, nb, 256, 0, st, a);
+  else if (G == 8) B200RL_LAUNCH(ppo_loss_cat_kernel<8>, nb, 256, 0, st, a);
+  else B200RL_LAUNCH(ppo_loss_cat_kernel<32>, nb, 256, 0, st, a);
+  B200RL_CHECK_LAUNCH("ppo_loss_categorical");
+  B200RL_LAUNCH(ppo_loss_final_kernel, 1, 512, 0, st, (const float*)workspace, (int)nb, (float)T * global_batch, (float)N, vf_coef, ent_coef, a.kl_terms, losses, nan_flag);
+  B200RL_CHECK_LAUNCH("ppo_loss_final");
+  return B200RL_OK;
+}
+
+int b200rl_categorical_logp(const float* logits, int64_t ld, const int32_t* action, int64_t N,
+                            int64_t A, float* out, int32_t* nan_flag, void* stream) {
+  B200RL_CHECK_ARG(logits && action && out && N >= 0 && A >= 1 && ld >= A,
+                   "categorical_logp: bad argument");
+  if (N == 0) return B200RL_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int G = cat_group(A);
+  const unsigned nb = cat_blocks(N, G, 1 << 30);
+  if (G == 1) B200RL_LAUNCH(categorical_logp_kernel<1>, nb, 256, 0, st, logits, ld, action, N, A, out, nan_flag);
+  else if (G == 8) B200RL_LAUNCH(categorical_logp_kernel<8>, nb, 256, 0, st, logits, ld, action, N, A, out, nan_flag);
+  else B200RL_LAUNCH(categorical_logp_kernel<32>, nb, 256, 0, st, logits, ld, action, N, A, out, nan_flag);
+  B200RL_CHECK_LAUNCH("categorical_logp");
+  return B200RL_OK;
+}
+
+int b200rl_ppo_kl_categorical(const float* logits, int64_t ld, const float* old_logits,
+                              int64_t ld_old, const float* w, int64_t N, int64_t A,
+                              float out_scale, float* out_kl, float* out_sum, void* workspace,
+                              int64_t ws_bytes, void* stream) {
+  B200RL_CHECK_ARG(logits && old_logits && out_sum, "ppo_kl_categorical: NULL argument");
+  B200RL_CHECK_ARG(N >= 1 && A >= 1 && ld >= A && ld_old >= A, "ppo_kl_categorical: bad sizes");
+  B200RL_CHECK_ARG(workspace && ws_bytes >= (int64_t)(kCatRedBlocks * sizeof(float)),
+                   "ppo_kl_categorical: workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int G = cat_group(A);
+  const unsigned nb = cat_blocks(N, G, kCatRedBlocks);
+  float* part = (float*)workspace;
+  if (G == 1) B200RL_LAUNCH(ppo_kl_cat_partial_kernel<1>, nb, 256, 0, st, logits, ld, old_logits, ld_old, w, N, A, out_kl, part);
+  else if (G == 8) B200RL_LAUNCH(ppo_kl_cat_partial_kernel<8>, nb, 256, 0, st, logits, ld, old_logits, ld_old, w, N, A, out_kl, part);
+  else B200RL_LAUNCH(ppo_kl_cat_partial_kernel<32>, nb, 256, 0, st, logits, ld, old_logits, ld_old, w, N, A, out_kl, part);
+  B200RL_CHECK_LAUNCH("ppo_kl_categorical_partial");
+  B200RL_LAUNCH(ppo_kl_final_kernel, 1, 512, 0, st, (const float*)workspace, (int)nb, out_scale, out_sum);
+  B200RL_CHECK_LAUNCH("ppo_kl_final");
+  return B200RL_OK;
+}
+
+int b200rl_categorical_sample(const float* logits, int64_t ld, int64_t N, int64_t A,
+                              uint64_t seed, uint64_t* rng_call_dev, int32_t* out, void* stream) {
+  B200RL_CHECK_ARG(logits && out && rng_call_dev && N >= 1 && A >= 1 && ld >= A,
+                   "categorical_sample: bad argument");
+  B200RL_LAUNCH(categorical_sample_kernel, blocks_for(N), 256, 0, (cudaStream_t)stream, logits, ld, N, A, seed, rng_call_dev, out);
+  B200RL_CHECK_LAUNCH("categorical_sample");
   return B200RL_OK;
 }
 

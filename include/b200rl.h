@@ -266,6 +266,44 @@ int b200rl_normal_logp(const float* loc, const float* scale, int64_t ld, const f
 int b200rl_normal_sample(const float* loc, const float* scale, int64_t ld, int64_t N, int64_t A,
                          const float* amin, const float* amax, uint64_t seed,
                          uint64_t* rng_call_dev, float* out, void* stream);
+/* Categorical policy (discrete actions; CategoricalProjectionNetwork logits,
+ * networks/categorical_projection_network.py).  Logits are [N, A] with row stride ld; actions are
+ * int32 in [0, A).  An action outside [0, A) is clamped for the read and sets *nan_flag = 1
+ * (nan_flag may be NULL), so check_numerics() reports it.
+ * b200rl_ppo_loss_categorical is the twin of b200rl_ppo_loss: same old_logp / adv / ret / v /
+ * v_old / w inputs, clipping semantics, losses[6] layout and workspace; log p = log_softmax(z)[a]
+ * (max-subtracted), entropy = -sum p log p; dlogits (row stride ld_g) = g_logp (1[j=a] - p_j)
+ * + g_ent (-p_j (log p_j + H)) + g_kl (p_j - q_j), q = softmax(old_logits). */
+typedef struct {
+  const float* old_logits; /* device [N, A], row stride ld_old: the behaviour policy */
+  int64_t ld_old;
+  const float* terms;      /* device float[3] from b200rl_ppo_kl_terms */
+  float grad_scale;        /* d(mean_kl)/d(sum_n w_n kl_n) = 1 / N_global */
+} b200rl_ppo_kl_logits_t;
+int b200rl_ppo_loss_categorical(const float* logits, int64_t ld, const int32_t* action,
+                                const float* old_logp, const float* adv, const float* ret,
+                                const float* v, const float* v_old, const float* w, int64_t N,
+                                int64_t A, int64_t T, float global_batch, float clip_eps,
+                                float value_clip, float vf_coef, float ent_coef, float logp_clip,
+                                float* losses, float* dlogits, int64_t ld_g, float* dv,
+                                int32_t* nan_flag, const b200rl_ppo_kl_logits_t* kl,
+                                void* workspace, int64_t ws_bytes, void* stream);
+/* Behaviour log-probs log_softmax(logits)[action] (counterpart of b200rl_normal_logp). */
+int b200rl_categorical_logp(const float* logits, int64_t ld, const int32_t* action, int64_t N,
+                            int64_t A, float* out, int32_t* nan_flag, void* stream);
+/* out_sum = out_scale * sum_n w_n * KL(Categorical(old_logits)_n || Categorical(logits)_n),
+ * KL = sum_j q_j (log q_j - log p_j) (tfp _kl_categorical_categorical); same two-stage
+ * reduction, out_kl and w conventions as b200rl_ppo_kl. */
+int b200rl_ppo_kl_categorical(const float* logits, int64_t ld, const float* old_logits,
+                              int64_t ld_old, const float* w, int64_t N, int64_t A,
+                              float out_scale, float* out_kl, float* out_sum, void* workspace,
+                              int64_t ws_bytes, void* stream);
+/* Collect-policy draw: u = uniform_f32(philox4x32_10(counter=(n, call), key=seed).x); the action is
+ * the smallest k with u < cdf_k, cdf the fp32 running sum in index order of
+ * exp(z - max) / sum exp(z - max), or A-1 if there is none.  rng_call_dev is uint64[2]
+ * {call, ticket}; every launch (and every graph replay) advances call. */
+int b200rl_categorical_sample(const float* logits, int64_t ld, int64_t N, int64_t A,
+                              uint64_t seed, uint64_t* rng_call_dev, int32_t* out, void* stream);
 /* NormalProjectionNetwork head (networks/normal_projection_network.py): loc = tanh-squash of the
  * mean layer to [amin, amax], scale = softplus(bias) broadcast; bwd returns dm_raw and the
  * per-element d(scale bias) terms (column-sum them with b200rl_colsum). */
