@@ -234,7 +234,12 @@ int b200rl_soft_update(float* target, const float* source, int64_t n, float tau,
   B200RL_CHECK_ARG(target && source && n >= 0, "soft_update: bad argument");
   B200RL_CHECK_ARG(tau >= 0.f && tau <= 1.f, "Input `tau` should be in [0, 1].");
   B200RL_CHECK_ARG(period <= 1 || counter_dev, "soft_update: period>1 needs a counter");
-  if (n == 0 || tau == 0.f) return B200RL_OK;  // utils/common.py:301-302 no-op
+  // tau == 0 or no variables: the blend is a no-op (utils/common.py:301-302), but a Periodically
+  // counter still advances on every call (assign_add before tf.cond, utils/common.py:494-497)
+  if (n == 0 || tau == 0.f) {
+    if (period <= 1) return B200RL_OK;
+    n = 0;
+  }
   B200RL_LAUNCH(soft_update_kernel, flat_grid(n), 256, 0, (cudaStream_t)stream, target, source, n, tau, period, counter_dev);
   B200RL_CHECK_LAUNCH("soft_update");
   return B200RL_OK;

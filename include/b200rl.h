@@ -463,7 +463,8 @@ int b200rl_rmsprop_tf(float* p, const float* g, float* ms, float* mg, float* mom
                       const float* grad_scale_dev, void* stream);
 /* soft_variables_update (utils/common.py:250-346): t = (1-tau)*t + tau*s, gated on device by
  * Periodically (utils/common.py:450-507): if period>1 the kernel does
- * c = ++(*counter_dev); update only when c % period == 0.  period<=1: always. */
+ * c = ++(*counter_dev); update only when c % period == 0.  period<=1: always.  tau == 0 leaves
+ * the target alone but still advances the counter. */
 int b200rl_soft_update(float* target, const float* source, int64_t n, float tau,
                        int64_t period, int64_t* counter_dev, void* stream);
 /* Per-variable clip_by_norm (utils/eager_utils.py:227-246): segments given by
