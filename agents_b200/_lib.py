@@ -106,6 +106,15 @@ SIGNATURES = {
     'b200rl_sac_actor_loss': [_P, _P, _P, _P, _P, c_i64, c_f32, c_f32, _P, _P, _P, _P, _P, _P],
     'b200rl_sac_alpha_loss': [_P, _P, _P, c_i64, c_f32, c_int, c_f32, c_f32, _P, _P, _P, _P],
     'b200rl_concat2': [_P, c_i64, c_i64, _P, c_i64, c_i64, c_i64, _P, _P],
+    'b200rl_cql_candidates': [_P, c_i64, c_i64, c_i64, c_i64, c_i64, _P, _P, _P, c_u64, _P, _P, _P,
+                              _P, _P],
+    'b200rl_cql_reward_noise': [_P, c_i64, _P, _P, c_u64, _P, _P, _P],
+    'b200rl_cql_loss': [_P, _P, _P, c_i64, c_i64, c_f32, c_f32, _P, _P, c_f32, c_f32, c_f32, c_int,
+                        _P, _P, _P, _P, _P, _P, _P, c_i64, _P],
+    'b200rl_cql_bc_actor_loss': [_P, _P, c_i64, _P, _P, _P, _P, _P, _P, c_i64, c_i64, c_i64, c_f32,
+                                 c_f32, _P, _P, _P, _P, _P],
+    'b200rl_cql_bc_actor_bwd': [_P, _P, c_i64, _P, _P, _P, _P, c_i64, c_i64, c_i64, c_f32, c_f32, _P,
+                                _P],
     'b200rl_nstep_reduce': [_P, _P, c_f64, _P, _P, c_i64, c_i64, _P],
     'b200rl_dqn_td_loss': [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_i64, c_i64, c_i64, c_i64, c_i64,
                            c_f64, c_f64, c_int, c_f32, _P, _P, _P, _P, _P, _P],

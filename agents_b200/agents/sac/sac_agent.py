@@ -31,6 +31,8 @@ from agents_b200.utils import common
 from agents_b200.utils import nest
 
 SacLossInfo = collections.namedtuple('SacLossInfo', ('critic_loss', 'actor_loss', 'alpha_loss'))
+_Batch = collections.namedtuple('_Batch', ('obs', 'obs2', 'action', 'reward', 'discount', 'weights',
+                                           'B', 'gb'))
 _SAC_SEED_TAG = 0x5341435F53414D50
 
 
@@ -159,6 +161,21 @@ class SacAgent(tf_agent.TFAgent):
     common.soft_variables_update(self._critic_params, self._target_params, tau=1.0)
 
   def _train(self, experience, weights=None, noise=None):
+    b = self._batch(experience, weights)
+    n_next = n_actor = n_alpha = None
+    if noise is not None:
+      n_next, n_actor, n_alpha = noise
+    closs = self._critic_step(b, n_next)
+    aloss = self._actor_step(b, n_actor)
+    alloss = self._alpha_step(b, n_alpha)
+    self._bump_train_step(1)
+    self._update_target()
+    total = closs + aloss + alloss
+    return tf_agent.LossInfo(total.reshape(()), SacLossInfo(closs.reshape(()), aloss.reshape(()),
+                                                            alloss.reshape(())))
+
+  def _batch(self, experience, weights):
+    """The [B, 2, ...] experience as the step tensors the three updates read."""
     if not isinstance(experience, trajectory.Trajectory):
       raise TypeError('Input type not supported: {}'.format(type(experience)))
     tf_agent.validate_trajectory(experience, self.training_data_spec, 2)
@@ -168,75 +185,94 @@ class SacAgent(tf_agent.TFAgent):
     reward = experience.reward[:, 0].float().contiguous()
     discount = experience.discount[:, 0].float().contiguous()
     B = reward.shape[0]
-    dev = reward.device
-    st = _lib.stream()
-    gb = float(B * self.replicas)
     if weights is not None:
-      weights = torch.as_tensor(weights, dtype=torch.float32, device=dev).expand(B).contiguous()
-    n_next = n_actor = n_alpha = None
-    if noise is not None:
-      n_next, n_actor, n_alpha = noise
-    c1, c2 = self._critic_network_1, self._critic_network_2
-    a_dim, o_dim = c1.act_dim, c1.obs_dim
-    new = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
+      weights = torch.as_tensor(weights, dtype=torch.float32,
+                                device=reward.device).expand(B).contiguous()
+    return _Batch(obs=obs, obs2=obs2, action=action, reward=reward, discount=discount,
+                  weights=weights, B=B, gb=float(B * self.replicas))
 
-    # ---- critic step (sac_agent.py:341-362, critic_loss :559-643) --------------------------
-    a2, logp2, _ = self._train_policy.sample(obs2, noise=n_next)
-    tq1, _ = self._target_critic_network_1((obs2, a2))
-    tq2, _ = self._target_critic_network_2((obs2, a2))
-    x = c1.joint_input(obs, action)
-    q1, tape1 = c1.forward_train_joint(x)
-    q2, tape2 = c2.forward_train_joint(x)
-    closs, dq1, dq2 = new(1), new(B, 1), new(B, 1)
-    _lib.call('b200rl_sac_critic_loss', _lib.ptr(q1), _lib.ptr(q2), _lib.ptr(tq1), _lib.ptr(tq2),
-              _lib.ptr(logp2), _lib.ptr(reward), _lib.ptr(discount), _lib.ptr(weights),
-              _lib.ptr(self._log_alpha), B, float(self._gamma), float(self._reward_scale_factor),
-              float(self._critic_loss_weight), gb, _lib.ptr(closs), _lib.ptr(dq1), _lib.ptr(dq2),
-              None, _lib.ptr(self._nan_flag), st)
-    c1.backward(tape1, dq1)
-    c2.backward(tape2, dq2)
+  def _new(self, *shape):
+    return torch.empty(shape, dtype=torch.float32, device=self._log_alpha.device)
+
+  def _next_targets(self, b, noise):
+    """a' ~ pi(.|s'), log pi(a'|s') and the two target-critic values at (s', a')."""
+    a2, logp2, _ = self._train_policy.sample(b.obs2, noise=noise)
+    tq1, _ = self._target_critic_network_1((b.obs2, a2))
+    tq2, _ = self._target_critic_network_2((b.obs2, a2))
+    return tq1, tq2, logp2
+
+  def _apply_critic_grads(self, tape1, dq1, tape2, dq2):
+    self._critic_network_1.backward(tape1, dq1)
+    self._critic_network_2.backward(tape2, dq2)
     if self._grad_sync is not None:
       self._grad_sync(self._critic_grads)
     self._critic_optimizer.apply_flat(self._critic_params, self._critic_grads)
 
-    # ---- actor step against the updated critics (:364-377, actor_loss :645-694) -----------
-    a, logp, (head, atape, u, eps) = self._train_policy.sample(obs, noise=n_actor, keep=True)
-    xa = c1.joint_input(obs, a)
+  def _critic_step(self, b, noise):
+    """sac_agent.py:341-362, critic_loss :559-643."""
+    c1, c2 = self._critic_network_1, self._critic_network_2
+    tq1, tq2, logp2 = self._next_targets(b, noise)
+    x = c1.joint_input(b.obs, b.action)
+    q1, tape1 = c1.forward_train_joint(x)
+    q2, tape2 = c2.forward_train_joint(x)
+    B = b.B
+    closs, dq1, dq2 = self._new(1), self._new(B, 1), self._new(B, 1)
+    _lib.call('b200rl_sac_critic_loss', _lib.ptr(q1), _lib.ptr(q2), _lib.ptr(tq1), _lib.ptr(tq2),
+              _lib.ptr(logp2), _lib.ptr(b.reward), _lib.ptr(b.discount), _lib.ptr(b.weights),
+              _lib.ptr(self._log_alpha), B, float(self._gamma), float(self._reward_scale_factor),
+              float(self._critic_loss_weight), b.gb, _lib.ptr(closs), _lib.ptr(dq1), _lib.ptr(dq2),
+              None, _lib.ptr(self._nan_flag), _lib.stream())
+    self._apply_critic_grads(tape1, dq1, tape2, dq2)
+    return closs
+
+  def _actor_loss_hook(self, b, head, logp, aloss, dqa1, dqa2):
+    """Runs after the SAC actor loss, before the critics' input gradients (CqlSacAgent: BC)."""
+
+  def _actor_dhead_hook(self, b, head, dhead):
+    """Runs after dL/dhead is written, before the actor backward (CqlSacAgent: BC)."""
+
+  def _actor_step(self, b, noise):
+    """Against the updated critics (:364-377, actor_loss :645-694)."""
+    c1, c2 = self._critic_network_1, self._critic_network_2
+    a_dim, o_dim = c1.act_dim, c1.obs_dim
+    B, st = b.B, _lib.stream()
+    a, logp, (head, atape, u, eps) = self._train_policy.sample(b.obs, noise=noise, keep=True)
+    xa = c1.joint_input(b.obs, a)
     qa1, t1 = c1.forward_train_joint(xa)
     qa2, t2 = c2.forward_train_joint(xa)
-    aloss, dlogp, dqa1, dqa2 = new(1), new(B), new(B, 1), new(B, 1)
+    aloss, dlogp, dqa1, dqa2 = self._new(1), self._new(B), self._new(B, 1), self._new(B, 1)
     _lib.call('b200rl_sac_actor_loss', _lib.ptr(qa1), _lib.ptr(qa2), _lib.ptr(logp),
-              _lib.ptr(weights), _lib.ptr(self._log_alpha), B, float(self._actor_loss_weight), gb,
-              _lib.ptr(aloss), _lib.ptr(dlogp), _lib.ptr(dqa1), _lib.ptr(dqa2),
+              _lib.ptr(b.weights), _lib.ptr(self._log_alpha), B, float(self._actor_loss_weight),
+              b.gb, _lib.ptr(aloss), _lib.ptr(dlogp), _lib.ptr(dqa1), _lib.ptr(dqa2),
               _lib.ptr(self._nan_flag), st)
+    self._actor_loss_hook(b, head, logp, aloss, dqa1, dqa2)
     _, dx1 = c1.backward(t1, dqa1, need_input_grad=True, need_param_grads=False)
     _, dx2 = c2.backward(t2, dqa2, need_input_grad=True, need_param_grads=False)
-    dhead = new(B, 2 * a_dim)
+    dhead = self._new(B, 2 * a_dim)
     _lib.call('b200rl_sac_sample_bwd', _lib.ptr(head), _lib.ptr(u), _lib.ptr(eps),
               _lib.ptr(self._actor_network.action_min), _lib.ptr(self._actor_network.action_max),
               dx1.data_ptr() + 4 * o_dim, dx2.data_ptr() + 4 * o_dim, o_dim + a_dim,
               _lib.ptr(dlogp), B, a_dim, _lib.ptr(dhead), st)
+    self._actor_dhead_hook(b, head, dhead)
     agrads = self._actor_network.backward(atape, dhead)
     if self._grad_sync is not None:
       self._grad_sync(agrads)
     self._actor_optimizer.apply_flat(self._actor_network.flat_params, agrads)
+    return aloss
 
-    # ---- alpha step against the updated actor (:379-390, alpha_loss :696-739) ---------------
-    _, logp3, _ = self._train_policy.sample(obs, noise=n_alpha)
-    alloss = new(1)
-    _lib.call('b200rl_sac_alpha_loss', _lib.ptr(logp3), _lib.ptr(weights),
-              _lib.ptr(self._log_alpha), B, float(self._target_entropy),
-              int(self._use_log_alpha_in_alpha_loss), float(self._alpha_loss_weight), gb,
-              _lib.ptr(alloss), _lib.ptr(self._dlog_alpha), _lib.ptr(self._nan_flag), st)
+  def _alpha_step(self, b, noise):
+    """Against the updated actor (:379-390, alpha_loss :696-739)."""
+    _, logp3, _ = self._train_policy.sample(b.obs, noise=noise)
+    alloss = self._new(1)
+    _lib.call('b200rl_sac_alpha_loss', _lib.ptr(logp3), _lib.ptr(b.weights),
+              _lib.ptr(self._log_alpha), b.B, float(self._target_entropy),
+              int(self._use_log_alpha_in_alpha_loss), float(self._alpha_loss_weight), b.gb,
+              _lib.ptr(alloss), _lib.ptr(self._dlog_alpha), _lib.ptr(self._nan_flag),
+              _lib.stream())
     if self._grad_sync is not None:
       self._grad_sync(self._dlog_alpha)
     self._alpha_optimizer.apply_flat(self._log_alpha, self._dlog_alpha)
-
-    self._bump_train_step(1)
-    self._update_target()
-    total = closs + aloss + alloss
-    return tf_agent.LossInfo(total.reshape(()), SacLossInfo(closs.reshape(()), aloss.reshape(()),
-                                                            alloss.reshape(())))
+    return alloss
 
   def check_numerics(self):
     if int(self._nan_flag.item()) != 0:

@@ -140,6 +140,39 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// ---- tanh-Normal helpers (sac.cu, cql.cu) --------------------------------------------------
+constexpr float kLog2PiS = 1.8378770664093453f;
+constexpr float kLog2 = 0.6931471805599453f;
+
+__device__ __forceinline__ float softplus_f(float x) {
+  return x > 20.f ? x : log1pf(expf(x));
+}
+
+// ---- row groups: a row of a [N, W] array handled by G lanes (lane l takes columns l, l+G, ...) --
+// Every warp runs the same number of row iterations (groups past N repeat their warp's first row
+// and discard the result), so the full-mask shuffles never diverge.
+template <int G>
+__device__ __forceinline__ float grp_max(float v) {
+#pragma unroll
+  for (int o = G / 2; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o, G));
+  return v;
+}
+template <int G>
+__device__ __forceinline__ float grp_sum(float v) {
+#pragma unroll
+  for (int o = G / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o, G);
+  return v;
+}
+
+// Row iteration shared by the group kernels: n is this group's row, n0 the row of the warp's first
+// group (warp-uniform loop bound).
+#define B200RL_GROUP_ROWS(G, N)                                                              \
+  const int lane = (int)(threadIdx.x % (G));                                                 \
+  const int64_t stride_ = (int64_t)gridDim.x * blockDim.x / (G);                             \
+  for (int64_t n = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / (G),                   \
+               n0 = ((int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) / (G);         \
+       n0 < (N); n += stride_, n0 += stride_)
+
 // Block-wide sum (blockDim.x multiple of 32, <= 1024). Deterministic order.
 __device__ __forceinline__ float block_sum(float v, float* smem32) {
   int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;

@@ -404,23 +404,9 @@ __global__ void ppo_kl_beta_update_kernel(const float* __restrict__ mean_kl,
 }
 
 // ---- Categorical policy (discrete actions): CategoricalProjectionNetwork logits [N, A] --------
-// A row of logits is handled by a group of G lanes (lane l takes columns l, l+G, ...); G follows
+// A row of logits is handled by a group of G lanes (B200RL_GROUP_ROWS, common.cuh); G follows
 // from A (cat_group): one thread per row for narrow rows, 8 or 32 lanes with shuffle reductions
-// for wide ones, so a row is read with coalesced loads.  Every warp runs the same number of row
-// iterations (groups past N repeat their warp's first row and discard the result), so the
-// full-mask shuffles never diverge.
-template <int G>
-__device__ __forceinline__ float grp_max(float v) {
-#pragma unroll
-  for (int o = G / 2; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o, G));
-  return v;
-}
-template <int G>
-__device__ __forceinline__ float grp_sum(float v) {
-#pragma unroll
-  for (int o = G / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o, G);
-  return v;
-}
+// for wide ones, so a row is read with coalesced loads.
 
 // Max-subtracted log-softmax statistics of one row: m = max z, s = sum exp(z - m),
 // t = sum exp(z - m) * (z - m).  log p_j = (z_j - m) - log s, entropy = log s - t / s.
@@ -440,15 +426,6 @@ __device__ __forceinline__ void row_softmax_stats(const float* __restrict__ z, i
   s = grp_sum<G>(s);
   t = grp_sum<G>(t);
 }
-
-// Row iteration shared by the group kernels: n is this group's row, n0 the row of the warp's first
-// group (warp-uniform loop bound).
-#define B200RL_GROUP_ROWS(G, N)                                                              \
-  const int lane = (int)(threadIdx.x % (G));                                                 \
-  const int64_t stride_ = (int64_t)gridDim.x * blockDim.x / (G);                             \
-  for (int64_t n = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / (G),                   \
-               n0 = ((int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) / (G);         \
-       n0 < (N); n += stride_, n0 += stride_)
 
 __device__ __forceinline__ int clamp_action(int32_t a, int64_t A, int32_t* nan_flag) {
   if (a < 0 || a >= A) {          // out-of-range action: read a valid column, report it

@@ -12,13 +12,6 @@
 
 namespace b200rl {
 
-constexpr float kLog2PiS = 1.8378770664093453f;
-constexpr float kLog2 = 0.6931471805599453f;
-
-__device__ __forceinline__ float softplus_f(float x) {
-  return x > 20.f ? x : log1pf(expf(x));
-}
-
 // head [N, 2A] = (loc | log_std).  u = loc + exp(log_std) * eps;  a = shift + half * tanh(u);
 // log_pi = sum_k [ -0.5 eps^2 - log_std - 0.5 log(2 pi) - log(half) - 2 (log2 - u - softplus(-2u)) ]
 __global__ void sac_sample_kernel(const float* __restrict__ head, int64_t N, int64_t A,

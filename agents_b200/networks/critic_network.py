@@ -40,11 +40,13 @@ class CriticNetwork(network.Network):
   def act_dim(self):
     return self._act_dim
 
-  def joint_input(self, observation, action):
-    """concat(observation, action) as one [N, D+A] buffer (either may be a strided view)."""
+  def joint_input(self, observation, action, out=None):
+    """concat(observation, action) as one [N, D+A] buffer (either may be a strided view), written
+    into the first N rows of `out` when given."""
     n = observation.shape[0]
-    out = torch.empty((n, self._obs_dim + self._act_dim), dtype=torch.float32,
-                      device=observation.device)
+    if out is None:
+      out = torch.empty((n, self._obs_dim + self._act_dim), dtype=torch.float32,
+                        device=observation.device)
     observation, action = observation.float(), action.float()
     lda = observation.stride(0) if observation.dim() == 2 and observation.stride(1) == 1 else None
     ldb = action.stride(0) if action.dim() == 2 and action.stride(1) == 1 else None

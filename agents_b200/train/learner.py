@@ -33,9 +33,11 @@ def _agent_state_tensors(agent):
     net = getattr(agent, name, None)
     if net is not None and hasattr(net, 'flat_params'):
       out[name] = net.flat_params
-  la = getattr(agent, '_log_alpha', None)
-  if isinstance(la, torch.Tensor):
-    out['_log_alpha'] = la
+  # SAC temperature; CQL-SAC's weight (a device scalar, or log_cql_alpha with Lagrange)
+  for name in ('_log_alpha', '_cql_alpha', '_log_cql_alpha'):
+    t = getattr(agent, name, None)
+    if isinstance(t, torch.Tensor):
+      out[name] = t
   # PPO: streaming normalisers (tf.Module variables of the agent in the reference, so they are
   # checkpointed and mirrored with it) and the adaptive KL coefficient (ppo_agent.py:341-343)
   for name in ('_observation_normalizer', '_reward_normalizer'):
@@ -52,7 +54,7 @@ def _agent_state_tensors(agent):
   # optimiser slots are created lazily on the first apply; materialise them for the parameter
   # buffers each agent steps, so that a freshly built agent can be restored into
   pairs = (('_optimizer', '_flat_params'), ('_critic_optimizer', '_critic_params'),
-           ('_alpha_optimizer', '_log_alpha'))
+           ('_alpha_optimizer', '_log_alpha'), ('_cql_alpha_optimizer', '_log_cql_alpha'))
   nets = (('_optimizer', '_q_network'), ('_actor_optimizer', '_actor_network'))
   for oname, pname in pairs:
     opt, p = getattr(agent, oname, None), getattr(agent, pname, None)
@@ -63,7 +65,8 @@ def _agent_state_tensors(agent):
     if hasattr(opt, '_get_slots') and net is not None and hasattr(net, 'flat_params') and \
         not isinstance(getattr(agent, '_flat_params', None), torch.Tensor):
       opt._get_slots(net.flat_params)
-  for oname in ('_optimizer', '_actor_optimizer', '_critic_optimizer', '_alpha_optimizer'):
+  for oname in ('_optimizer', '_actor_optimizer', '_critic_optimizer', '_alpha_optimizer',
+                '_cql_alpha_optimizer'):
     opt = getattr(agent, oname, None)
     if opt is not None and hasattr(opt, '_slots'):
       for i, slots in enumerate(opt._slots.values()):

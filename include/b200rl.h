@@ -374,6 +374,58 @@ int b200rl_concat2(const float* a, int64_t lda, int64_t da, const float* b, int6
                    int64_t db, int64_t N, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * CQL-SAC (csrc/cql.cu).  Replaces agents/cql/cql_sac_agent.py (_cql_loss :534-679, actor_loss
+ * :681-750, _get_cql_alpha :752-765, reward noise :832-839, the Lagrange step of _train
+ * :336-348).  The critic joint input x is [B + 2BN, D+A]: rows [0, B) (s, a_data), [B, B+BN) the
+ * policy candidates, [B+BN, B+2BN) the uniform candidates; row B + b*N + j belongs to state b.
+ * ------------------------------------------------------------------------------------ */
+/* Writes the observation columns of every candidate row of x, the action columns of the uniform
+ * rows (amin + u*(amax-amin), u in [0,1) from u_in [BN, A] (oracle mode) or Philox with
+ * rng_call_dev uint64[2] {call, ticket}), and head_tiled [BN, 2A] = head [B, 2A] repeated N times
+ * per row for b200rl_sac_sample, which then writes the policy rows' actions (ld_action = D+A). */
+int b200rl_cql_candidates(const float* obs, int64_t ld_obs, int64_t B, int64_t N, int64_t D,
+                          int64_t A, const float* amin, const float* amax, const float* u_in,
+                          uint64_t seed, uint64_t* rng_call_dev, const float* head, float* x,
+                          float* head_tiled, void* stream);
+/* out[B] = reward + stddev_dev[0] * z (z from z_in [B] or Philox + Box-Muller); out = reward while
+ * stddev_dev[0] <= 0.  The reference passes reward_noise_variance as the stddev. */
+int b200rl_cql_reward_noise(const float* reward, int64_t B, const float* stddev_dev,
+                            const float* z_in, uint64_t seed, uint64_t* rng_call_dev, float* out,
+                            void* stream);
+/* CQL(H) term on the critic outputs q1/q2 [B + 2BN] of the joint rows: lse_i = logsumexp over the
+ * 2N candidates of (temperature*Q_i - log density) / temperature (logp [BN] for the policy rows,
+ * uniform_logp for the uniform rows), cql_loss = mean_b[(lse_1 - q1) + (lse_2 - q2)] / 2.
+ * cql_alpha = exp(clip(log_cql_alpha_dev[0], clip_lo, clip_hi)) when log_cql_alpha_dev is given
+ * (Lagrange), else cql_alpha_dev[0].  Writes dq1/dq2 of the candidate rows, adds -cql_alpha/(2B)
+ * to rows [0, B) (overwrites them when bc_debug), and out[4] = {cql_loss, cql_alpha,
+ * critic_loss + cql_alpha*cql_loss (cql_alpha*cql_loss when bc_debug), cql_alpha_loss}; with
+ * Lagrange cql_alpha_loss = -cql_alpha*(cql_loss - cql_tau) and dlog_cql_alpha[0] its gradient
+ * (0 outside [clip_lo, clip_hi]), else cql_alpha_loss = 0.  workspace >= 256 floats. */
+int b200rl_cql_loss(const float* q1, const float* q2, const float* logp, int64_t B, int64_t N,
+                    float uniform_logp, float temperature, const float* cql_alpha_dev,
+                    const float* log_cql_alpha_dev, float clip_lo, float clip_hi, float cql_tau,
+                    int bc_debug, const float* critic_loss, float* dq1, float* dq2, float* out,
+                    float* dlog_cql_alpha, int32_t* nan_flag, void* workspace, int64_t ws_bytes,
+                    void* stream);
+/* Behavioural cloning while train_step_dev[0] < num_bc_steps (a no-op otherwise): replaces the SAC
+ * actor loss by loss_weight * sum(w*(exp(log_alpha)*logp - log pi(a_data|s))) / global_batch and
+ * zeroes dq1/dq2 [B].  log pi is the tanh-squashed Normal of head [B, 2A] at the dataset action
+ * (row stride ld_action), inverse tanh clipped to +-0.99999997. */
+int b200rl_cql_bc_actor_loss(const float* head, const float* action, int64_t ld_action,
+                             const float* amin, const float* amax, const float* logp,
+                             const float* weights, const float* log_alpha_dev,
+                             const int64_t* train_step_dev, int64_t num_bc_steps, int64_t B,
+                             int64_t A, float loss_weight, float global_batch, float* loss,
+                             float* dq1, float* dq2, int32_t* nan_flag, void* stream);
+/* Adds the BC term's d/dhead to dhead [B, 2A] (after b200rl_sac_sample_bwd wrote it) while
+ * train_step_dev[0] < num_bc_steps. */
+int b200rl_cql_bc_actor_bwd(const float* head, const float* action, int64_t ld_action,
+                            const float* amin, const float* amax, const float* weights,
+                            const int64_t* train_step_dev, int64_t num_bc_steps, int64_t B,
+                            int64_t A, float loss_weight, float global_batch, float* dhead,
+                            void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Network layers (fp32).  Replace Keras Dense/Conv2D fwd+bwd that the reference executes
  * through TensorFlow (networks/encoding_network.py:224-312, q_network.py:126-135).
  * All matrices are row-major.
