@@ -99,6 +99,8 @@ SIGNATURES = {
     'b200rl_normalizer_update': [_P, _P, _P, _P, _P, _P, c_f32, c_i64, _P],
     'b200rl_ppo_discounts': [_P, _P, c_f32, c_i64, _P, _P],
     'b200rl_ppo_weights': [_P, _P, _P, _P, c_i64, _P, _P],
+    'b200rl_reinforce_loss': [_P, _P, c_i64, _P, c_i64, _P, _P, _P, _P, _P, c_i64, c_i64, c_int,
+                              c_int, c_f32, c_f32, _P, _P, _P, c_i64, _P, _P, _P, _P, c_i64, _P],
     'b200rl_sac_sample': [_P, c_i64, c_i64, _P, _P, _P, c_u64, _P, _P, c_i64, _P, _P, _P, _P],
     'b200rl_sac_sample_bwd': [_P, _P, _P, _P, _P, _P, _P, c_i64, _P, c_i64, c_i64, _P, _P],
     'b200rl_sac_critic_loss': [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_i64, c_f32, c_f32, c_f32,

@@ -1,6 +1,7 @@
 // Shared device/host helpers for libb200rl (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -172,6 +173,34 @@ __device__ __forceinline__ float grp_sum(float v) {
   for (int64_t n = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / (G),                   \
                n0 = ((int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) / (G);         \
        n0 < (N); n += stride_, n0 += stride_)
+
+// ---- Categorical rows (ppo.cu, reinforce.cu) ---------------------------------------------------
+// Max-subtracted log-softmax statistics of one row: m = max z, s = sum exp(z - m),
+// t = sum exp(z - m) * (z - m).  log p_j = (z_j - m) - log s, entropy = log s - t / s.
+template <int G>
+__device__ __forceinline__ void row_softmax_stats(const float* __restrict__ z, int64_t A, int lane,
+                                                  float& m, float& s, float& t) {
+  m = -INFINITY;
+  for (int64_t j = lane; j < A; j += G) m = fmaxf(m, z[j]);
+  m = grp_max<G>(m);
+  s = 0.f; t = 0.f;
+  for (int64_t j = lane; j < A; j += G) {
+    const float d = z[j] - m;
+    const float e = expf(d);
+    s += e;
+    t += e > 0.f ? e * d : 0.f;
+  }
+  s = grp_sum<G>(s);
+  t = grp_sum<G>(t);
+}
+
+__device__ __forceinline__ int clamp_action(int32_t a, int64_t A, int32_t* nan_flag) {
+  if (a < 0 || a >= A) {          // out-of-range action: read a valid column, report it
+    if (nan_flag) *nan_flag = 1;
+    a = a < 0 ? 0 : (int32_t)(A - 1);
+  }
+  return a;
+}
 
 // Block-wide sum (blockDim.x multiple of 32, <= 1024). Deterministic order.
 __device__ __forceinline__ float block_sum(float v, float* smem32) {

@@ -406,34 +406,8 @@ __global__ void ppo_kl_beta_update_kernel(const float* __restrict__ mean_kl,
 // ---- Categorical policy (discrete actions): CategoricalProjectionNetwork logits [N, A] --------
 // A row of logits is handled by a group of G lanes (B200RL_GROUP_ROWS, common.cuh); G follows
 // from A (cat_group): one thread per row for narrow rows, 8 or 32 lanes with shuffle reductions
-// for wide ones, so a row is read with coalesced loads.
-
-// Max-subtracted log-softmax statistics of one row: m = max z, s = sum exp(z - m),
-// t = sum exp(z - m) * (z - m).  log p_j = (z_j - m) - log s, entropy = log s - t / s.
-template <int G>
-__device__ __forceinline__ void row_softmax_stats(const float* __restrict__ z, int64_t A, int lane,
-                                                  float& m, float& s, float& t) {
-  m = -INFINITY;
-  for (int64_t j = lane; j < A; j += G) m = fmaxf(m, z[j]);
-  m = grp_max<G>(m);
-  s = 0.f; t = 0.f;
-  for (int64_t j = lane; j < A; j += G) {
-    const float d = z[j] - m;
-    const float e = expf(d);
-    s += e;
-    t += e > 0.f ? e * d : 0.f;
-  }
-  s = grp_sum<G>(s);
-  t = grp_sum<G>(t);
-}
-
-__device__ __forceinline__ int clamp_action(int32_t a, int64_t A, int32_t* nan_flag) {
-  if (a < 0 || a >= A) {          // out-of-range action: read a valid column, report it
-    if (nan_flag) *nan_flag = 1;
-    a = a < 0 ? 0 : (int32_t)(A - 1);
-  }
-  return a;
-}
+// for wide ones, so a row is read with coalesced loads.  row_softmax_stats / clamp_action live in
+// common.cuh (shared with reinforce.cu).
 
 struct PpoCatArgs {
   const float* logits; int64_t ld;                           // current policy Categorical(logits)

@@ -1,0 +1,93 @@
+"""ActorPolicy (tf_agents/policies/actor_policy.py): actions from the distribution an
+ActorDistributionNetwork emits.
+
+collect=True  -> a draw from the distribution: Normal(loc, scale) through b200rl_normal_sample,
+                 clipped to the action spec when `clip` (the reference's clip=True default), or
+                 Categorical(logits) through b200rl_categorical_sample (`clip` does not apply).
+collect=False -> the greedy policy, the mode of the distribution: loc for a Normal, the first
+                 argmax of the logits for a Categorical (b200rl_epsilon_greedy with epsilon 0).
+Draws use a device {call, ticket} counter, so a captured collect step draws fresh values on every
+replay.  Subclasses record extra `policy_info` through `_info` (PPOPolicy).
+"""
+import torch
+
+from agents_b200 import _lib
+from agents_b200.policies import tf_policy
+from agents_b200.trajectories import policy_step
+from agents_b200.utils import nest
+
+_ACTOR_SEED_TAG = 0x4143544F52504F4C
+
+
+class ActorPolicy(tf_policy.TFPolicy):
+
+  _SEED_TAG = _ACTOR_SEED_TAG
+
+  def __init__(self, time_step_spec, action_spec, actor_network, clip=True, collect=True, seed=0,
+               info_spec=()):
+    if getattr(actor_network, 'state_spec', ()):
+      raise NotImplementedError('ActorPolicy supports stateless actor networks only.')
+    super().__init__(time_step_spec, action_spec, info_spec=info_spec)
+    self._actor_net = actor_network
+    self._clip, self._collect = clip, collect
+    self._seed = (int(seed) ^ self._SEED_TAG) & 0xFFFFFFFFFFFFFFFF
+    self._rng = None
+    self._action_spec_leaf = nest.flatten(action_spec)[0]
+
+  @property
+  def actor_network(self):
+    return self._actor_net
+
+  def variables(self):
+    return self._actor_net.variables
+
+  def _normalized(self, observation):
+    return observation
+
+  def distribution_params(self, time_step):
+    return self._actor_net.distribution_params(self._normalized(time_step.observation))
+
+  def _rng_block(self, device):
+    if self._rng is None or self._rng.device != device:
+      self._rng = torch.zeros(2, dtype=torch.int64, device=device)
+    return self._rng
+
+  def _categorical_action(self, logits):
+    n, a = logits.shape
+    act = torch.empty(n, dtype=torch.int32, device=logits.device)
+    if self._collect:
+      _lib.call('b200rl_categorical_sample', _lib.ptr(logits), a, n, a, self._seed,
+                _lib.ptr(self._rng_block(logits.device)), _lib.ptr(act), _lib.stream())
+    else:       # mode of the Categorical: the first argmax (epsilon 0 never picks at random)
+      _lib.call('b200rl_epsilon_greedy', _lib.ptr(logits), None, n, a, 0.0, self._seed,
+                _lib.ptr(self._rng_block(logits.device)), None, None, _lib.ptr(act),
+                _lib.stream())
+    spec = self._action_spec_leaf
+    act = act.reshape((n,) + tuple(spec.shape))
+    if spec.dtype != torch.int32:
+      act = act.to(spec.dtype)
+    return act
+
+  def _normal_action(self, loc, scale):
+    if not self._collect:
+      return loc
+    n, a = loc.shape
+    act = torch.empty_like(loc)
+    _lib.call('b200rl_normal_sample', _lib.ptr(loc), _lib.ptr(scale), a, n, a,
+              _lib.ptr(self._actor_net.action_min) if self._clip else None,
+              _lib.ptr(self._actor_net.action_max) if self._clip else None, self._seed,
+              _lib.ptr(self._rng_block(loc.device)), _lib.ptr(act), _lib.stream())
+    return act
+
+  def _info(self, observation, params):
+    """policy_info of a step; `params` are the distribution parameters."""
+    return ()
+
+  def _action(self, time_step, policy_state, seed):
+    obs = self._normalized(time_step.observation)
+    params = self._actor_net.distribution_params(obs)
+    if self._actor_net.discrete:
+      act = self._categorical_action(params)
+    else:
+      act = self._normal_action(*params)
+    return policy_step.PolicyStep(act, policy_state, self._info(obs, params))

@@ -28,7 +28,7 @@ def _agent_state_tensors(agent):
   """Flat parameter / slot tensors that define the agent's state (for mirroring + checkpoints)."""
   out = {}
   for name in ('_q_network', '_target_q_network', '_actor_net', '_value_net', '_actor_network',
-               '_critic_network_1', '_critic_network_2', '_target_critic_network_1',
+               '_value_network', '_critic_network_1', '_critic_network_2', '_target_critic_network_1',
                '_target_critic_network_2'):
     net = getattr(agent, name, None)
     if net is not None and hasattr(net, 'flat_params'):

@@ -334,6 +334,37 @@ int b200rl_ppo_weights(const int32_t* step_type, const float* ret, const float* 
                        const float* weights, int64_t n, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * REINFORCE loss — agents/reinforce/reinforce_agent.py:48-80 (_standard_normalize,
+ * _entropy_loss), :321-379 (masks, num_episodes, advantages), :442-567 (losses).
+ * Over a batch-major [B, T] batch, N = B*T rows (N < 2^24):
+ *   weights = user weights (NULL: 1) * valid, valid[b,t] = some t' >= t of row b has
+ *             next_step_type == LAST; num_episodes = sum(next_step_type == LAST)
+ *   adv     = returns - value (use_advantage) or returns; normalize: (adv - mean) /
+ *             (sqrt(var) + float32 eps), moments over all N entries
+ *   pg      = -sum log pi(a|s) (step_type != LAST) adv * weights / num_episodes
+ *   entropy = entropy_coef * mean_N(-H weights) (entropy_coef 0: 0)
+ *   value   = value_coef * sum (returns - value)^2 weights / num_episodes (value NULL: 0)
+ * The distribution is Normal(p0 = loc, p1 = scale), [N, A] views with row stride ld, with float
+ * actions [N, A] and gradients d0 = dloc, d1 = dscale (row stride ld_g); or, when p1 and d1 are
+ * NULL, Categorical(p0 = logits) with int32 actions [N] and d0 = dlogits.
+ * value / dvalue [N] (both or neither): dvalue includes d(pg)/d(value) through the advantage
+ * (value predictions are not stop-gradient there); where sigma = 0 the normalisation's
+ * d(sigma) term is defined as 0.
+ * losses[6] = {policy_gradient, policy_network_regularization (0), entropy_regularization,
+ * value_estimation, value_network_regularization (0), total}; the caller adds the L2 terms.
+ * num_episodes (optional) gets the count on the device.  *flag is OR-ed with 1 when the total is
+ * not finite or an action is outside [0, A) (it is clamped for the read), and with 2 when there
+ * is no complete episode (then every loss and gradient is 0).  No host reads.
+ * ws_bytes >= 4 * (4096 + round_up(B, 4) + N). */
+int b200rl_reinforce_loss(const float* p0, const float* p1, int64_t ld, const void* action,
+                          int64_t A, const float* returns, const float* value,
+                          const int32_t* step_type, const int32_t* next_step_type,
+                          const float* weights, int64_t B, int64_t T, int use_advantage,
+                          int normalize, float entropy_coef, float value_coef, float* losses,
+                          float* d0, float* d1, int64_t ld_g, float* dvalue, float* num_episodes,
+                          int32_t* flag, void* workspace, int64_t ws_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * SAC update math — agents/sac/sac_agent.py, sac/tanh_normal_projection_network.py,
  * distributions/utils.py (SquashToSpecNormal), distributions/tanh_bijector_stable.py
  * ------------------------------------------------------------------------------------ */
