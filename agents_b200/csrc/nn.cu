@@ -48,9 +48,11 @@ struct FastDiv {
 
 // Operand views.  Every view is separable: element (row, k) lives at row_off(row) + k_off(k),
 // where "row" is m for A views and n for B views.  kKContig says which index is contiguous in
-// memory (4 consecutive k can then be fetched with one 16-byte / 4-byte vector load when
-// vec4_ok()).  `at` is the scalar accessor used by the fp32 FFMA kernel.
+// memory (4 consecutive elements along it can then be copied as one 16-byte / 4-byte chunk when
+// vec4_ok()).  `at` is the scalar accessor used by the fp32 FFMA kernel; the tensor-core kernel
+// copies raw Elem values from addr() and converts them to fp32 with cvt().
 struct ARow {
+  using Elem = float;
   const float* p;
   int64_t ld;
   static constexpr bool kKContig = true;
@@ -59,11 +61,11 @@ struct ARow {
   __device__ __forceinline__ int64_t row_off(int64_t m) const { return m * ld; }
   __device__ __forceinline__ int64_t k_off(int64_t k) const { return k; }
   __device__ __forceinline__ bool vec4_ok() const { return (ld & 3) == 0 && ((uintptr_t)p & 15) == 0; }
-  __device__ __forceinline__ float ld1(int64_t off) const { return p[off]; }
-  __device__ __forceinline__ float4 ld4(int64_t off) const { return *reinterpret_cast<const float4*>(p + off); }
+  __device__ __forceinline__ float cvt(Elem x) const { return x; }
   __device__ __forceinline__ const void* addr(int64_t off) const { return p + off; }
 };
 struct ACol {
+  using Elem = float;
   const float* p;
   int64_t ld;
   static constexpr bool kKContig = false;
@@ -72,11 +74,11 @@ struct ACol {
   __device__ __forceinline__ int64_t row_off(int64_t m) const { return m; }
   __device__ __forceinline__ int64_t k_off(int64_t k) const { return k * ld; }
   __device__ __forceinline__ bool vec4_ok() const { return (ld & 3) == 0 && ((uintptr_t)p & 15) == 0; }
-  __device__ __forceinline__ float ld1(int64_t off) const { return p[off]; }
-  __device__ __forceinline__ float4 ld4(int64_t off) const { return *reinterpret_cast<const float4*>(p + off); }
+  __device__ __forceinline__ float cvt(Elem x) const { return x; }
   __device__ __forceinline__ const void* addr(int64_t off) const { return p + off; }
 };
 struct BRow {  // B(k, n) = p[k*ld + n]  (n contiguous)
+  using Elem = float;
   const float* p;
   int64_t ld;
   static constexpr bool kNContig = true;
@@ -86,11 +88,11 @@ struct BRow {  // B(k, n) = p[k*ld + n]  (n contiguous)
   __device__ __forceinline__ int64_t row_off(int64_t n) const { return n; }
   __device__ __forceinline__ int64_t k_off(int64_t k) const { return k * ld; }
   __device__ __forceinline__ bool vec4_ok() const { return (ld & 3) == 0 && ((uintptr_t)p & 15) == 0; }
-  __device__ __forceinline__ float ld1(int64_t off) const { return p[off]; }
-  __device__ __forceinline__ float4 ld4(int64_t off) const { return *reinterpret_cast<const float4*>(p + off); }
+  __device__ __forceinline__ float cvt(Elem x) const { return x; }
   __device__ __forceinline__ const void* addr(int64_t off) const { return p + off; }
 };
 struct BCol {  // B(k, n) = p[n*ld + k]  (k contiguous)
+  using Elem = float;
   const float* p;
   int64_t ld;
   static constexpr bool kNContig = false;
@@ -100,8 +102,7 @@ struct BCol {  // B(k, n) = p[n*ld + k]  (k contiguous)
   __device__ __forceinline__ int64_t row_off(int64_t n) const { return n * ld; }
   __device__ __forceinline__ int64_t k_off(int64_t k) const { return k; }
   __device__ __forceinline__ bool vec4_ok() const { return (ld & 3) == 0 && ((uintptr_t)p & 15) == 0; }
-  __device__ __forceinline__ float ld1(int64_t off) const { return p[off]; }
-  __device__ __forceinline__ float4 ld4(int64_t off) const { return *reinterpret_cast<const float4*>(p + off); }
+  __device__ __forceinline__ float cvt(Elem x) const { return x; }
   __device__ __forceinline__ const void* addr(int64_t off) const { return p + off; }
 };
 
@@ -144,29 +145,19 @@ struct ConvView {
   __device__ __forceinline__ bool vec4_ok() const {
     return (g.C & 3) == 0 && (g.in_img & 3) == 0 && ((uintptr_t)x & (4 * sizeof(T) - 1)) == 0;
   }
-  __device__ __forceinline__ float4 load4(int64_t off) const;
   // tensor-core path: x * (1/scale) instead of the IEEE division (differs by <= 1 ulp; the
-  // parity bar is 1e-5, and the division costs ~25 instructions per element in the producers)
-  __device__ __forceinline__ float load_fast(int64_t off) const;
+  // parity bar is 1e-5, and the division costs ~25 instructions per element in the split)
+  __device__ __forceinline__ float cvt_fast(T v) const;
 };
 template <>
-__device__ __forceinline__ float4 ConvView<float>::load4(int64_t off) const {
-  return *reinterpret_cast<const float4*>(x + off);
-}
+__device__ __forceinline__ float ConvView<float>::cvt_fast(float v) const { return v; }
 template <>
-__device__ __forceinline__ float4 ConvView<uint8_t>::load4(int64_t off) const {
-  const uchar4 u = *reinterpret_cast<const uchar4*>(x + off);
-  const float inv = __frcp_rn(scale);
-  return make_float4((float)u.x * inv, (float)u.y * inv, (float)u.z * inv, (float)u.w * inv);
-}
-template <>
-__device__ __forceinline__ float ConvView<float>::load_fast(int64_t off) const { return x[off]; }
-template <>
-__device__ __forceinline__ float ConvView<uint8_t>::load_fast(int64_t off) const {
-  return (float)x[off] * __frcp_rn(scale);
+__device__ __forceinline__ float ConvView<uint8_t>::cvt_fast(uint8_t v) const {
+  return (float)v * __frcp_rn(scale);
 }
 template <typename T>
 struct AConv {
+  using Elem = T;
   ConvView<T> v;
   static constexpr bool kKContig = true;
   static constexpr bool kExact = false;
@@ -176,12 +167,12 @@ struct AConv {
   __device__ __forceinline__ int64_t row_off(int64_t m) const { return v.pos_offset((uint32_t)m); }
   __device__ __forceinline__ int64_t k_off(int64_t k) const { return v.patch_offset((uint32_t)k); }
   __device__ __forceinline__ bool vec4_ok() const { return v.vec4_ok(); }
-  __device__ __forceinline__ float ld1(int64_t off) const { return v.load_fast(off); }
-  __device__ __forceinline__ float4 ld4(int64_t off) const { return v.load4(off); }
+  __device__ __forceinline__ float cvt(Elem x) const { return v.cvt_fast(x); }
   __device__ __forceinline__ const void* addr(int64_t off) const { return v.x + off; }
 };
 template <typename T>
 struct AConvT {
+  using Elem = T;
   ConvView<T> v;
   static constexpr bool kKContig = false;
   static constexpr bool kExact = false;
@@ -191,14 +182,14 @@ struct AConvT {
   __device__ __forceinline__ int64_t row_off(int64_t m) const { return v.patch_offset((uint32_t)m); }
   __device__ __forceinline__ int64_t k_off(int64_t k) const { return v.pos_offset((uint32_t)k); }
   __device__ __forceinline__ bool vec4_ok() const { return v.vec4_ok(); }
-  __device__ __forceinline__ float ld1(int64_t off) const { return v.load_fast(off); }
-  __device__ __forceinline__ float4 ld4(int64_t off) const { return v.load4(off); }
+  __device__ __forceinline__ float cvt(Elem x) const { return v.cvt_fast(x); }
   __device__ __forceinline__ const void* addr(int64_t off) const { return v.x + off; }
 };
 
 // Raw uint8 pixel views for the tensor-core path: values 0..255 are exact in TF32, the 1/scale of
 // the reference's cast+/255 layer is applied to the accumulator in the epilogue instead.
 struct AConvU8Raw {
+  using Elem = uint8_t;
   ConvView<uint8_t> v;
   static constexpr bool kKContig = true;
   static constexpr bool kExact = true;
@@ -206,14 +197,11 @@ struct AConvU8Raw {
   __device__ __forceinline__ int64_t row_off(int64_t m) const { return v.pos_offset((uint32_t)m); }
   __device__ __forceinline__ int64_t k_off(int64_t k) const { return v.patch_offset((uint32_t)k); }
   __device__ __forceinline__ bool vec4_ok() const { return v.vec4_ok(); }
-  __device__ __forceinline__ float ld1(int64_t off) const { return (float)v.x[off]; }
-  __device__ __forceinline__ float4 ld4(int64_t off) const {
-    const uchar4 u = *reinterpret_cast<const uchar4*>(v.x + off);
-    return make_float4((float)u.x, (float)u.y, (float)u.z, (float)u.w);
-  }
+  __device__ __forceinline__ float cvt(Elem x) const { return (float)x; }
   __device__ __forceinline__ const void* addr(int64_t off) const { return v.x + off; }
 };
 struct AConvTU8Raw {
+  using Elem = uint8_t;
   ConvView<uint8_t> v;
   static constexpr bool kKContig = false;
   static constexpr bool kExact = true;
@@ -221,11 +209,7 @@ struct AConvTU8Raw {
   __device__ __forceinline__ int64_t row_off(int64_t m) const { return v.patch_offset((uint32_t)m); }
   __device__ __forceinline__ int64_t k_off(int64_t k) const { return v.pos_offset((uint32_t)k); }
   __device__ __forceinline__ bool vec4_ok() const { return v.vec4_ok(); }
-  __device__ __forceinline__ float ld1(int64_t off) const { return (float)v.x[off]; }
-  __device__ __forceinline__ float4 ld4(int64_t off) const {
-    const uchar4 u = *reinterpret_cast<const uchar4*>(v.x + off);
-    return make_float4((float)u.x, (float)u.y, (float)u.z, (float)u.w);
-  }
+  __device__ __forceinline__ float cvt(Elem x) const { return (float)x; }
   __device__ __forceinline__ const void* addr(int64_t off) const { return v.x + off; }
 };
 

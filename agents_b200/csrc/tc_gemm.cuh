@@ -4,22 +4,23 @@
 //   C[M,N] (+)= act(A[M,K] @ B[K,N] + bias)      A, B given as operand views (see nn.cu)
 //
 // Why 3xTF32: north_star parity is 1e-5 relative on the loss; one TF32 pass keeps ~11 mantissa
-// bits (1e-3).  Each fp32 operand x is split in registers into hi = x with the low 13 mantissa
-// bits cleared and lo = x - hi (exact); the tensor core accumulates lo_a*hi_b + hi_a*lo_b +
-// hi_a*hi_b into the same fp32 accumulator (the dropped lo*lo term is 2^-22 relative).
+// bits (1e-3).  Each fp32 operand x is split into hi = x with the low 13 mantissa bits cleared
+// and lo = x - hi (exact); the tensor core accumulates lo_a*hi_b + hi_a*lo_b + hi_a*hi_b into the
+// same fp32 accumulator (the dropped lo*lo term is 2^-22 relative).
 //
 // Structure (one CTA = one 128 x BN output tile, 256 threads = two warpgroups):
-//   every thread gathers its share of a (128 x 32) A tile and a (BN x 32) B^T tile through the
-//   operand views (implicit im2col, u8->f32 cast and transposes happen here; the global loads of
-//   K block i+1 are in flight while block i is split and stored), splits hi/lo and stores them
-//   K-major into 128B-swizzled shared memory, the layout wgmma reads (tf32 operands must be
-//   K-major, so MN-contiguous views are transposed on the way in);
-//   after one CTA barrier per K block, warpgroup w issues wgmma.m64nBNk8 for rows 64w..64w+63
-//   (4 K steps x up to 3 passes per 32-wide K block) and keeps one group in flight while the
-//   next block is stored: three stages make one barrier per K block sufficient (the stage
-//   written in block i was last read by the MMAs of block i-3, which every warpgroup retired
-//   before the barrier of block i-1).
-//   The epilogue parks the accumulators in the idle stage buffers and drains them row-per-thread:
+//   operand ring: every thread copies its share of the raw (128 x 32) A tile and (BN x 32) B^T
+//   tile of a K block global -> shared with cp.async (16-byte chunks, 4-byte ones for uint8 and
+//   misaligned views; zero-fill through src-size past every tail), kRing - 1 K blocks ahead of the
+//   block being multiplied, so several blocks of loads are in flight at once;
+//   per K block: wait for the block's copies, barrier, issue the copies of block i + kRing - 1,
+//   then split: read the raw tile from shared memory (u8 -> f32 conversion here), write TF32 hi /
+//   lo K-major into 128B-swizzled planes, the layout wgmma reads (tf32 operands must be K-major,
+//   so MN-contiguous views are transposed in this pass); a second barrier, then warpgroup w
+//   issues wgmma.m64nBNk8 for rows 64w..64w+63 (4 K steps x up to 3 passes per 32-wide K block)
+//   and keeps one group in flight while the next block is split.  Two plane stages: the first
+//   barrier of block i comes after every warpgroup retired the MMAs of block i-2.
+//   The epilogue parks the accumulators in the idle planes / ring and drains them row-per-thread:
 //   bias / activation / act' mask / split-K partials, the fused col2im scatter-add, or red.add.
 #pragma once
 #include <cuda_runtime.h>
@@ -31,7 +32,11 @@ namespace tc {
 constexpr int kBM = 128;
 constexpr int kBK = 32;                    // fp32 elements = 128 bytes = one swizzle row
 constexpr int kThreads = 256;
-constexpr int kStages = 3;
+constexpr int kPlaneStages = 2;           // TF32 hi / lo planes the MMAs read
+constexpr int kMaxRing = 8;               // raw operand stages (K blocks) in the cp.async ring
+constexpr int kSmemOptIn = 227 * 1024;    // sm_90: dynamic shared memory one CTA may opt into
+constexpr int kSmemPerSM = 228 * 1024;
+constexpr int kSmemPerCta = 1024;         // reserved by the system for every resident CTA
 constexpr int kChainBlocks = 8;           // K blocks per tensor-core accumulation chain (CHAINS)
 
 // optional phase stamps (b200rl_tc_debug_buffer): [block][8] nanosecond timers
@@ -147,6 +152,9 @@ __device__ __forceinline__ void split_store1(unsigned char* hi_tile, unsigned ch
 
 // A_EXACT: the A view yields values that are exactly representable in TF32 (raw uint8 pixels), so
 // A needs no "lo" plane and the product needs only 2 passes (a*b_lo + a*b_hi).
+// Shared memory: [kPlaneStages x split planes][kRing x raw operand tiles][bias slice].  The ring is
+// as deep as the opt-in limit allows (at most kMaxRing); a layout whose ring can still be >= 4
+// deep in half an SM runs 2 CTAs per SM (kCtasPerSM, the kernel's launch bound).
 template <int BN, int PASSES, bool A_EXACT = false>
 struct SmemLayout {
   static constexpr int kATile = kBM * 128;
@@ -154,107 +162,193 @@ struct SmemLayout {
   static constexpr int kNumA = (PASSES == 3 && !A_EXACT) ? 2 : 1;   // A planes
   static constexpr int kNumB = PASSES == 3 ? 2 : 1;                 // B planes
   static constexpr int kStage = kNumA * kATile + kNumB * kBTile;
+  static constexpr int kPlanes = kPlaneStages * kStage;
+  // raw tiles sized for the larger (MN-contiguous, padded) layout; A_EXACT views are uint8
+  static constexpr int kRawA = kBK * (kBM * (A_EXACT ? 1 : 4) + 16);
+  static constexpr int kRawB = kBK * (BN * 4 + 16);
+  static constexpr int kRawStage = kRawA + kRawB;
+  static constexpr int kFixed = kPlanes + 1024 /*alignment slack*/ + BN * 4 /*bias*/;
+  static constexpr int kRing2 = (kSmemPerSM / 2 - kSmemPerCta - kFixed) / kRawStage;
+  static constexpr int kCtasPerSM = kRing2 >= 4 ? 2 : 1;
+  static constexpr int kRingFit = kCtasPerSM == 2 ? kRing2 : (kSmemOptIn - kFixed) / kRawStage;
+  static constexpr int kRing = kRingFit < kMaxRing ? kRingFit : kMaxRing;
+  static_assert(kRing >= 2, "the operand ring needs two stages");
   static constexpr int kPitch = BN + 4;                             // epilogue staging row (floats)
-  static_assert(kBM * kPitch * 4 <= kStages * kStage, "epilogue staging tile must fit");
-  static constexpr int kBytes = kStages * kStage + 1024 /*alignment slack*/ + BN * 4 /*bias*/;
+  static_assert(kBM * kPitch * 4 <= kPlanes + kRing * kRawStage, "epilogue staging tile must fit");
+  static constexpr int kBytes = kFixed + kRing * kRawStage;
 };
 
-// One chunk = 4 consecutive k of one row.  roff = view.row_off(row); koff[i] = view.k_off(k+i).
+// ---- operand ring: global -> shared with cp.async, then split from shared memory -------------
+// One chunk = 4 consecutive elements along the contiguous index of a view (k for K-contiguous
+// views, m / n for MN-contiguous ones): 16 bytes of fp32 or 4 bytes of uint8.  When the view is
+// vec4_ok() a chunk is one cp.async whose src-size covers only the in-range elements; the rest of
+// the 16 / 4 bytes is zero-filled by the copy, so nothing past a K tail, a row end or an image is
+// ever read.  Otherwise every element moves on its own (4-byte cp.async for fp32, a plain byte
+// load and store for uint8, which cp.async cannot copy).
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+template <int BYTES>
+__device__ __forceinline__ void cp_async(uint32_t dst, const void* src, uint32_t src_bytes) {
+  if constexpr (BYTES == 16)
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes)
+                 : "memory");
+  else
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(src_bytes)
+                 : "memory");
+}
+// n of the chunk's 4 elements (0..4) are in range and contiguous from `off`
 template <class V>
-__device__ __forceinline__ float4 load_chunk(const V& v, int64_t roff, bool row_ok, int64_t k,
-                                             int64_t ke, const int64_t (&koff)[4], bool full_vec) {
-  float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (!row_ok || k >= ke) return r;
-  if (full_vec) return v.ld4(roff + koff[0]);
-  r.x = v.ld1(roff + koff[0]);
-  if (k + 1 < ke) r.y = v.ld1(roff + koff[1]);
-  if (k + 2 < ke) r.z = v.ld1(roff + koff[2]);
-  if (k + 3 < ke) r.w = v.ld1(roff + koff[3]);
-  return r;
+__device__ __forceinline__ void copy_chunk(const V& v, uint32_t dst, int64_t off, int n) {
+  constexpr int E = sizeof(typename V::Elem);
+  cp_async<4 * E>(dst, v.addr(n > 0 ? off : 0), (uint32_t)(n * E));
+}
+template <class V>
+__device__ __forceinline__ void copy_elem(const V& v, uint32_t dst, int64_t off, bool ok) {
+  if constexpr (sizeof(typename V::Elem) == 4) {
+    cp_async<4>(dst, v.addr(ok ? off : 0), ok ? 4u : 0u);
+  } else {
+    const uint32_t x = ok ? *static_cast<const uint8_t*>(v.addr(off)) : 0u;
+    asm volatile("st.shared.u8 [%0], %1;" ::"r"(dst), "r"(x) : "memory");
+  }
+}
+// 4 raw elements of a chunk in shared memory -> fp32 (uint8 views convert here)
+template <class V>
+__device__ __forceinline__ float4 ld_raw4(const V& v, uint32_t saddr) {
+  if constexpr (sizeof(typename V::Elem) == 4) {
+    float4 x;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                 : "=f"(x.x), "=f"(x.y), "=f"(x.z), "=f"(x.w) : "r"(saddr) : "memory");
+    return x;
+  } else {
+    uint32_t w;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w) : "r"(saddr) : "memory");
+    return make_float4(v.cvt((uint8_t)w), v.cvt((uint8_t)(w >> 8)), v.cvt((uint8_t)(w >> 16)),
+                       v.cvt((uint8_t)(w >> 24)));
+  }
 }
 
-// A [ROWS x 32] fp32 operand tile is moved in two steps so that the global loads of K block i+1
-// are in flight while block i is split and stored: gather (global -> registers) and scatter
-// (registers -> hi/lo planes in 128B-swizzled shared memory).
-// K-contiguous views: thread = (row group tid>>3, chunk tid&7), 8 lanes read 128 contiguous
-// bytes of a row; row_offs[i] belongs to row (tid>>3) + 32 i.
+// Raw tile of a (ROWS x 32) operand block.  K-contiguous views: chunk j of row r sits where the
+// split planes keep it (sw128 for fp32, 32-byte rows for uint8), so the split pass reads and writes
+// the same conflict-free pattern.  MN-contiguous views: 32 k-rows of ROWS elements, 16 bytes of
+// padding per k-row so that the 8 k-rows a quarter-warp reads in the transposing split fall into
+// different banks.
+template <class V, int ROWS>
+struct RawTile {
+  static constexpr int E = sizeof(typename V::Elem);
+  static constexpr int kPitch = ROWS * E + 16;   // MN-contiguous k-row
+  __device__ static __forceinline__ uint32_t k_chunk(uint32_t r, uint32_t j) {
+    return E == 4 ? sw128(r, j) : r * 32u + j * 4u;
+  }
+};
+
+// K-contiguous views: thread = (row group tid>>3, chunk tid&7), 8 lanes copy one row's 32 k;
+// row_offs[i] belongs to row (tid>>3) + 32 i (hoisted once per CTA).
 template <int ROWS, class V>
-__device__ __forceinline__ void gather_tile(const V& v, const int64_t* row_offs,
-                                            uint32_t row_ok_mask, int64_t k0, int64_t ke, bool vec,
-                                            int tid, float4 (&val)[ROWS * 8 / kThreads]) {
+__device__ __forceinline__ void copy_tile_k(const V& v, uint32_t dst, const int64_t* row_offs,
+                                            uint32_t row_ok_mask, int64_t k0, int64_t ke,
+                                            bool vec, int tid) {
+  using R = RawTile<V, ROWS>;
   constexpr int NV = ROWS * 8 / kThreads;
   const int j = tid & 7;
   const int64_t k = k0 + j * 4;
-  const bool full_vec = vec && (k + 3 < ke);
-  int64_t koff[4];
-  koff[0] = k < ke ? v.k_off(k) : 0;
+  const int nk = k < ke ? (ke - k < 4 ? (int)(ke - k) : 4) : 0;
+  if (vec) {
+    const int64_t ko = nk > 0 ? v.k_off(k) : 0;
 #pragma unroll
-  for (int i = 1; i < 4; ++i) koff[i] = (!full_vec && k + i < ke) ? v.k_off(k + i) : 0;
+    for (int i = 0; i < NV; ++i) {
+      const uint32_t r = (uint32_t)((tid >> 3) + 32 * i);
+      copy_chunk(v, dst + R::k_chunk(r, j), row_offs[i] + ko, ((row_ok_mask >> i) & 1u) ? nk : 0);
+    }
+  } else {
+    int64_t ko[4];
 #pragma unroll
-  for (int i = 0; i < NV; ++i)
-    val[i] = load_chunk(v, row_offs[i], (row_ok_mask >> i) & 1u, k, ke, koff, full_vec);
+    for (int e = 0; e < 4; ++e) ko[e] = e < nk ? v.k_off(k + e) : 0;
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+      const uint32_t r = (uint32_t)((tid >> 3) + 32 * i);
+      const bool ok = (row_ok_mask >> i) & 1u;
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        copy_elem(v, dst + R::k_chunk(r, j) + e * R::E, row_offs[i] + ko[e], ok && e < nk);
+    }
+  }
 }
 
-template <int ROWS, bool WITH_LO>
-__device__ __forceinline__ void scatter_tile(unsigned char* hi, unsigned char* lo, int tid,
-                                             const float4 (&val)[ROWS * 8 / kThreads]) {
+// MN-contiguous views: chunk c = tid + 256 i is rows 4 (c % CPR) .. +3 at k = c / CPR, so a warp
+// copies whole 4*CPR-element runs of a k-row and a thread keeps one row group (roff = the view's
+// row offset of that group's first row, nrow = how many of its 4 rows are in range).
+template <int ROWS, class V>
+__device__ __forceinline__ void copy_tile_mn(const V& v, uint32_t dst, int64_t r, int64_t roff,
+                                             int nrow, int64_t k0, int64_t ke, bool vec, int tid) {
+  using R = RawTile<V, ROWS>;
+  constexpr int CPR = ROWS / 4, NV = ROWS * 8 / kThreads;
+  static_assert(kThreads % CPR == 0, "a thread's row group must not change between its chunks");
+  const uint32_t cm = (uint32_t)(tid % CPR);
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const int kk = (tid + kThreads * i) / CPR;
+    const int64_t k = k0 + kk;
+    const bool kok = k < ke;
+    const uint32_t d = dst + (uint32_t)kk * R::kPitch + cm * 4u * R::E;
+    if (vec) {
+      copy_chunk(v, d, roff + (kok ? v.k_off(k) : 0), kok ? nrow : 0);
+    } else {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const bool ok = kok && e < nrow;
+        copy_elem(v, d + e * R::E, ok ? v.row_off(r + e) + v.k_off(k) : 0, ok);
+      }
+    }
+  }
+}
+
+// Split pass of K-contiguous tiles: raw chunk (r, j) -> TF32 hi / lo at sw128(r, j).
+template <int ROWS, bool WITH_LO, class V>
+__device__ __forceinline__ void split_tile_k(const V& v, uint32_t raw, unsigned char* hi,
+                                             unsigned char* lo, int tid) {
+  using R = RawTile<V, ROWS>;
   constexpr int NV = ROWS * 8 / kThreads;
 #pragma unroll
-  for (int i = 0; i < NV; ++i)
-    split_store<WITH_LO>(hi, lo, sw128((uint32_t)((tid >> 3) + 32 * i), (uint32_t)(tid & 7)), val[i]);
+  for (int i = 0; i < NV; ++i) {
+    const uint32_t r = (uint32_t)((tid >> 3) + 32 * i), j = (uint32_t)(tid & 7);
+    split_store<WITH_LO>(hi, lo, sw128(r, j), ld_raw4(v, raw + R::k_chunk(r, j)));
+  }
 }
 
-// MN-contiguous views (the M/N index is contiguous in memory): chunk c = tid + 256 i holds rows
-// 4 cm .. 4 cm + 3 at reduction index k, with k & 7 = c & 7, cm = (c >> 3) % CPR and
-// k >> 3 = (c >> 3) / CPR.  A warp reads 8 k-rows x 64 contiguous bytes; the transposing scalar
-// stores of a warp then spread over 16 banks (2-way conflicts instead of 16-way for a
-// row-per-lane map).  cm does not depend on i, so every chunk of a thread covers the same 4
-// columns (the fused bias gradient relies on it).
+// Split pass of MN-contiguous tiles, transposed to K-major on the way: chunk c = tid + 256 i holds
+// rows 4 cm .. 4 cm + 3 at reduction index k, with k & 7 = c & 7, cm = (c >> 3) % CPR and
+// k >> 3 = (c >> 3) / CPR.  The transposing scalar stores of a warp then spread over 16 banks
+// (2-way conflicts instead of 16-way for a row-per-lane map).  cm does not depend on i, so every
+// chunk of a thread covers the same 4 columns: `colsum` accumulates their sums (fused bias
+// gradient).
 template <int ROWS>
 struct MnMap {
   static constexpr int CPR = ROWS / 4;
   __device__ static __forceinline__ int cm(int c) { return (c >> 3) % CPR; }
   __device__ static __forceinline__ int kk(int c) { return (c & 7) | (((c >> 3) / CPR) << 3); }
 };
-template <int ROWS, class V>
-__device__ __forceinline__ void gather_tile_mn(const V& v, int64_t row0, int64_t row_limit,
-                                               int64_t k0, int64_t ke, bool vec, int tid,
-                                               float4 (&val)[ROWS * 8 / kThreads]) {
-  constexpr int NV = ROWS * 8 / kThreads;
-  const int64_t r = row0 + 4 * MnMap<ROWS>::cm(tid);
-  const int64_t roff = r < row_limit ? v.row_off(r) : 0;
-  const bool row_full = r + 3 < row_limit;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int64_t k = k0 + MnMap<ROWS>::kk(tid + kThreads * i);
-    float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (k < ke && r < row_limit) {
-      const int64_t off = roff + v.k_off(k);
-      if (vec && row_full) {
-        x = v.ld4(off);
-      } else {
-        x.x = v.ld1(off);
-        if (r + 1 < row_limit) x.y = v.ld1(v.row_off(r + 1) + v.k_off(k));
-        if (r + 2 < row_limit) x.z = v.ld1(v.row_off(r + 2) + v.k_off(k));
-        if (r + 3 < row_limit) x.w = v.ld1(v.row_off(r + 3) + v.k_off(k));
-      }
-    }
-    val[i] = x;
-  }
-}
-template <int ROWS, bool WITH_LO>
-__device__ __forceinline__ void scatter_tile_mn(unsigned char* hi, unsigned char* lo, int tid,
-                                                const float4 (&val)[ROWS * 8 / kThreads]) {
+template <int ROWS, bool WITH_LO, class V>
+__device__ __forceinline__ void split_tile_mn(const V& v, uint32_t raw, unsigned char* hi,
+                                              unsigned char* lo, int tid, bool do_colsum,
+                                              float4& colsum) {
+  using R = RawTile<V, ROWS>;
   constexpr int NV = ROWS * 8 / kThreads;
   const uint32_t r = 4u * (uint32_t)MnMap<ROWS>::cm(tid);
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const uint32_t k = (uint32_t)MnMap<ROWS>::kk(tid + kThreads * i);
+    const float4 x = ld_raw4(v, raw + k * R::kPitch + r * R::E);
+    if (do_colsum) {
+      colsum.x += x.x; colsum.y += x.y; colsum.z += x.z; colsum.w += x.w;
+    }
     const uint32_t j = k >> 2, e = (k & 3u) * 4u;
-    split_store1<WITH_LO>(hi, lo, sw128(r + 0, j) + e, val[i].x);
-    split_store1<WITH_LO>(hi, lo, sw128(r + 1, j) + e, val[i].y);
-    split_store1<WITH_LO>(hi, lo, sw128(r + 2, j) + e, val[i].z);
-    split_store1<WITH_LO>(hi, lo, sw128(r + 3, j) + e, val[i].w);
+    split_store1<WITH_LO>(hi, lo, sw128(r + 0, j) + e, x.x);
+    split_store1<WITH_LO>(hi, lo, sw128(r + 1, j) + e, x.y);
+    split_store1<WITH_LO>(hi, lo, sw128(r + 2, j) + e, x.z);
+    split_store1<WITH_LO>(hi, lo, sw128(r + 3, j) + e, x.w);
   }
 }
 
@@ -278,20 +372,15 @@ struct EpiArgs {
 // AL / BL are the fp32 operand views of nn.cu (row index = m for A, n for B).
 // CHAINS: the K range of a CTA is long (> kChainBlocks blocks), see `sum` below.
 template <int BN, int PASSES, int EPI, class AL, class BL, bool CHAINS>
-__global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const BL b,
-                                                              const EpiArgs epi,
-                                                              float* __restrict__ C,
-                                                              const float* __restrict__ bias,
-                                                              int64_t M, int64_t N, int64_t K,
-                                                              int act, int beta, int splits,
-                                                              int64_t k_per_split,
-                                                              float* __restrict__ ws,
-                                                              float out_scale) {
+__global__ void __launch_bounds__(kThreads, SmemLayout<BN, PASSES, AL::kExact>::kCtasPerSM)
+tc_gemm_kernel(const AL a, const BL b, const EpiArgs epi, float* __restrict__ C,
+               const float* __restrict__ bias, int64_t M, int64_t N, int64_t K, int act, int beta,
+               int splits, int64_t k_per_split, float* __restrict__ ws, float out_scale) {
   using L = SmemLayout<BN, PASSES, AL::kExact>;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  float* sbias = reinterpret_cast<float*>(smem + kStages * L::kStage);   // bias slice / column sums
+  float* sbias = reinterpret_cast<float*>(smem + L::kPlanes + L::kRing * L::kRawStage);   // bias / column sums
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int wg = tid >> 7;                                  // warpgroup: tile rows 64 wg ..
@@ -313,18 +402,26 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const 
   constexpr int NRA = AL::kKContig ? kBM * 8 / kThreads : 1;
   constexpr int NRB = BL::kKContig ? BN * 8 / kThreads : 1;
   static_assert(BN * 8 >= kThreads, "BN must be >= 32");
+  // hoisted row offsets (the implicit-im2col index math runs once per CTA).  K-contiguous views:
+  // row (tid>>3) + 32 i; MN-contiguous views: the 4-row group of copy_tile_mn.
   int64_t a_off[NRA], b_off[NRB];
   uint32_t a_ok = 0, b_ok = 0;
-  if (AL::kKContig) {
+  int64_t a_r = 0, b_r = 0;
+  int a_nrow = 0, b_nrow = 0;
+  if constexpr (AL::kKContig) {
 #pragma unroll
-    for (int i = 0; i < NRA; ++i) {  // hoisted row offsets (implicit-im2col index math runs once)
+    for (int i = 0; i < NRA; ++i) {
       const int r = (tid >> 3) + 32 * i;
       const bool ok = m0 + r < M;
       a_off[i] = ok ? a.row_off(m0 + r) : 0;
       a_ok |= (ok ? 1u : 0u) << i;
     }
+  } else {
+    a_r = m0 + 4 * (tid % (kBM / 4));
+    a_nrow = M - a_r < 0 ? 0 : (M - a_r < 4 ? (int)(M - a_r) : 4);
+    a_off[0] = a_nrow > 0 ? a.row_off(a_r) : 0;
   }
-  if (BL::kKContig) {
+  if constexpr (BL::kKContig) {
 #pragma unroll
     for (int i = 0; i < NRB; ++i) {
       const int r = (tid >> 3) + 32 * i;
@@ -332,20 +429,29 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const 
       b_off[i] = ok ? b.row_off(n0 + r) : 0;
       b_ok |= (ok ? 1u : 0u) << i;
     }
+  } else {
+    b_r = n0 + 4 * (tid % (BN / 4));
+    b_nrow = N - b_r < 0 ? 0 : (N - b_r < 4 ? (int)(N - b_r) : 4);
+    b_off[0] = b_nrow > 0 ? b.row_off(b_r) : 0;
   }
   const bool a_vec = a.vec4_ok(), b_vec = b.vec4_ok();
-  constexpr int NVA = kBM * 8 / kThreads, NVB = BN * 8 / kThreads;
-  float4 av[NVA], bv[NVB], an[NVA], bn[NVB];
-  auto gather_a = [&](int64_t k0, float4 (&dst)[NVA]) {
-    if constexpr (AL::kKContig) gather_tile<kBM>(a, a_off, a_ok, k0, ke, a_vec, tid, dst);
-    else gather_tile_mn<kBM>(a, m0, M, k0, ke, a_vec, tid, dst);
+  const uint32_t smem_base = smem_addr(smem);
+  const uint32_t ring_base = smem_base + L::kPlanes;
+  // Copies K block `blk` into its ring slot; commits a (possibly empty) group either way, so that
+  // the group count stays in step with the block index.
+  auto issue = [&](int blk) {
+    if (blk < nkb) {
+      const uint32_t slot = ring_base + (uint32_t)(blk % L::kRing) * L::kRawStage;
+      const int64_t k0 = kb + (int64_t)blk * kBK;
+      if constexpr (AL::kKContig) copy_tile_k<kBM>(a, slot, a_off, a_ok, k0, ke, a_vec, tid);
+      else copy_tile_mn<kBM>(a, slot, a_r, a_off[0], a_nrow, k0, ke, a_vec, tid);
+      if constexpr (BL::kKContig) copy_tile_k<BN>(b, slot + L::kRawA, b_off, b_ok, k0, ke, b_vec, tid);
+      else copy_tile_mn<BN>(b, slot + L::kRawA, b_r, b_off[0], b_nrow, k0, ke, b_vec, tid);
+    }
+    cp_async_commit();
   };
-  auto gather_b = [&](int64_t k0, float4 (&dst)[NVB]) {
-    if constexpr (BL::kKContig) gather_tile<BN>(b, b_off, b_ok, k0, ke, b_vec, tid, dst);
-    else gather_tile_mn<BN>(b, n0, N, k0, ke, b_vec, tid, dst);
-  };
-  // bias gradient fused into the weight-gradient GEMM: B = dY[k, n] is read by these threads
-  // anyway; in the MN-major gather every chunk of a thread covers the same 4 columns, so one
+  // bias gradient fused into the weight-gradient GEMM: B = dY[k, n] passes through these threads
+  // in the split; in the MN-major map every chunk of a thread covers the same 4 columns, so one
   // float4 per thread accumulates the column sums of the CTA's K range.
   const bool do_colsum = EPI == EPI_ATOMIC && !BL::kKContig && epi.colsum != nullptr &&
                          blockIdx.y == 0;
@@ -361,37 +467,28 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const 
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
 #pragma unroll
   for (int i = 0; i < (CHAINS ? BN / 2 : 1); ++i) sum[i] = 0.f;
-  if (nkb > 0) {
-    gather_a(kb, av);
-    gather_b(kb, bv);
-  }
-  const uint32_t smem_base = smem_addr(smem);
-  // One K block: issue the NEXT block's global loads into `nxt`, split/store `cur`, barrier, MMAs.
-  // The two register sets swap roles every block (loop unrolled by two below) -- copying
-  // nxt -> cur at the end of the body would wait for the loads that were just issued.
-  auto k_block = [&](int kbi, float4 (&cur_a)[NVA], float4 (&cur_b)[NVB], float4 (&nxt_a)[NVA],
-                     float4 (&nxt_b)[NVB]) {
-    const int s = kbi % kStages;
-    if (kbi + 1 < nkb) {
-      const int64_t k1 = kb + (int64_t)(kbi + 1) * kBK;
-      gather_a(k1, nxt_a);
-      gather_b(k1, nxt_b);
-    }
+  // the ring's first kRing - 1 blocks are in flight before the loop starts
+#pragma unroll 1
+  for (int blk = 0; blk < L::kRing - 1; ++blk) issue(blk);
+#pragma unroll 1
+  for (int kbi = 0; kbi < nkb; ++kbi) {
+    // this thread's copies of block kbi have landed; the barrier makes everyone's visible, and it
+    // frees the ring slot of block kbi - 1 (split before the last barrier) and plane stage
+    // kbi % 2 (its MMAs, block kbi - 2, retired in every warpgroup's wait_group 1 below)
+    cp_async_wait<L::kRing - 2>();
+    __syncthreads();
+    issue(kbi + L::kRing - 1);
+    const int s = kbi % kPlaneStages;
+    const uint32_t raw = ring_base + (uint32_t)(kbi % L::kRing) * L::kRawStage;
     unsigned char* st = smem + s * L::kStage;
     unsigned char* a_hi = st;
     unsigned char* a_lo = st + L::kATile;
     unsigned char* b_hi = st + L::kNumA * L::kATile;
     unsigned char* b_lo = b_hi + L::kBTile;
-    if constexpr (AL::kKContig) scatter_tile<kBM, kLoA>(a_hi, a_lo, tid, cur_a);
-    else scatter_tile_mn<kBM, kLoA>(a_hi, a_lo, tid, cur_a);
-    if constexpr (BL::kKContig) scatter_tile<BN, kLo>(b_hi, b_lo, tid, cur_b);
-    else scatter_tile_mn<BN, kLo>(b_hi, b_lo, tid, cur_b);
-    if (do_colsum) {
-#pragma unroll
-      for (int i = 0; i < NVB; ++i) {
-        bsum.x += cur_b[i].x; bsum.y += cur_b[i].y; bsum.z += cur_b[i].z; bsum.w += cur_b[i].w;
-      }
-    }
+    if constexpr (AL::kKContig) split_tile_k<kBM, kLoA>(a, raw, a_hi, a_lo, tid);
+    else split_tile_mn<kBM, kLoA>(a, raw, a_hi, a_lo, tid, false, bsum);
+    if constexpr (BL::kKContig) split_tile_k<BN, kLo>(b, raw + L::kRawA, b_hi, b_lo, tid);
+    else split_tile_mn<BN, kLo>(b, raw + L::kRawA, b_hi, b_lo, tid, do_colsum, bsum);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic stores -> async proxy
     __syncthreads();
     const uint32_t sa = smem_base + (uint32_t)s * L::kStage + (uint32_t)wg * (64u * 128u);
@@ -400,7 +497,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const 
     const bool fresh = CHAINS && kbi % kChainBlocks == 0;   // first block of a chain
     if constexpr (CHAINS) {
       if (fresh && kbi > 0) {
-        // the previous block's MMAs ran during this block's gather/scatter; usually retired
+        // the previous block's MMAs ran during this block's split; usually retired
         wgmma_wait<0>();
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) sum[i] += acc[i];
@@ -424,11 +521,6 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const AL a, const 
     }
     wgmma_commit();
     wgmma_wait<1>();
-  };
-#pragma unroll 1
-  for (int kbi = 0; kbi < nkb; kbi += 2) {
-    k_block(kbi, av, bv, an, bn);
-    if (kbi + 1 < nkb) k_block(kbi + 1, an, bn, av, bv);
   }
   wgmma_wait<0>();
   if constexpr (CHAINS) {
