@@ -120,6 +120,9 @@ SIGNATURES = {
     'b200rl_nstep_reduce': [_P, _P, c_f64, _P, _P, c_i64, c_i64, _P],
     'b200rl_dqn_td_loss': [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_i64, c_i64, c_i64, c_i64, c_i64,
                            c_f64, c_f64, c_int, c_f32, _P, _P, _P, _P, _P, _P],
+    'b200rl_c51_loss': [_P, _P, _P, _P, c_i64, _P, _P, _P, _P, c_i64, c_i64, c_i64, c_i64, c_f32,
+                        c_f32, c_f32, _P, _P, _P, _P, c_i64, _P],
+    'b200rl_c51_q_values': [_P, _P, c_i64, c_i64, c_i64, _P, _P],
     'b200rl_set_gemm_mode': [c_int],
     'b200rl_tc_debug_buffer': [_P],
     'b200rl_dense_fwd': [_P, c_i64, _P, _P, _P, c_i64, c_i64, c_i64, c_int, _P, c_i64, _P],

@@ -54,6 +54,7 @@ class DqnAgent(tf_agent.TFAgent):
 
   _DOUBLE_Q = False          # select the bootstrap action with the online network
   _SELECT_UNMASKED = False   # D3qn: raw argmax over the selector's output (no action constraints)
+  _FUSED_TD_LOSS = True      # False: td_errors_loss_fn is accepted but not used (CategoricalDqnAgent)
 
   def __init__(self, time_step_spec, action_spec, q_network, optimizer,
                observation_and_action_constraint_splitter=None, epsilon_greedy=0.1,
@@ -90,7 +91,7 @@ class DqnAgent(tf_agent.TFAgent):
     self._n_step_update = n_step_update
     self._optimizer = optimizer
     self._td_errors_loss_fn = td_errors_loss_fn or common.element_wise_huber_loss
-    self._loss_kind = _loss_kind(self._td_errors_loss_fn)
+    self._loss_kind = _loss_kind(self._td_errors_loss_fn) if self._FUSED_TD_LOSS else None
     self._gamma = gamma
     self._reward_scale_factor = reward_scale_factor
     self._gradient_clipping = gradient_clipping

@@ -195,6 +195,38 @@ int b200rl_dqn_td_loss(const float* q, const float* next_q_tgt, const float* nex
                        float* dq, int32_t* nan_flag, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * Categorical DQN (C51) loss, forward + backward -- agents/categorical_dqn/
+ * categorical_dqn_agent.py:271-556 (+ project_distribution :562-731).
+ *   q, next_q [B, A*N]  online logits at s_0 / target logits at s_n (row-major head output)
+ *   next_mask [B, A]    optional int32 action constraint at s_n (0 = masked)
+ *   actions, action_stride: column 0 of the [B, T] action tensor, read in place; actions
+ *                       outside [0, A) are clamped and set *nan_flag
+ *   reward/discount [B, T] raw trajectory fields; support[N] the atoms (equally spaced) of
+ *                       the projection; select_support[N] (optional, default support) the atoms
+ *                       of the target policy's expected Q, which picks the greedy action
+ *                       (categorical_q_policy.py:141-144 builds them with np.linspace)
+ *   2 <= N <= 1024, T >= 2.  global_batch: divisor of the loss sum.
+ *   workspace: >= 4*B bytes of device scratch (per-row losses).
+ * Outputs: loss[0] = sum_b CE_b / global_batch (no reg, no sample weights), dq[B, A*N] =
+ *          dLoss/dq (zero outside the taken action's N atoms), nan_flag (optional int32, set
+ *          when the loss is not finite or an action was out of range).
+ * Fixed-order reductions: repeated calls on the same input return the same bits.
+ * ------------------------------------------------------------------------------------ */
+int b200rl_c51_loss(const float* q, const float* next_q, const int32_t* next_mask,
+                    const int32_t* actions, int64_t action_stride, const float* reward,
+                    const float* discount, const float* support,
+                    const float* select_support, int64_t B, int64_t A, int64_t N, int64_t T,
+                    float gamma, float reward_scale, float global_batch, float* loss,
+                    float* dq, int32_t* nan_flag, void* workspace, int64_t ws_bytes,
+                    void* stream);
+
+/* Expected Q of categorical logits (common.convert_q_logits_to_values,
+ * policies/categorical_q_policy.py:174-180): q[b, a] = sum_j support[j] softmax(logits[b, a, :])_j
+ * for logits [B, A*N]; the result feeds b200rl_epsilon_greedy. */
+int b200rl_c51_q_values(const float* logits, const float* support, int64_t B, int64_t A,
+                        int64_t N, float* q, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * Episodic replay buffer bookkeeping -- replay_buffers/episodic_replay_buffer.py.
  * An episode slot owns rows [slot*max_len, (slot+1)*max_len) of the leaf storage; row
  * capacity*max_len is a trash row for items whose episode id is stale.
