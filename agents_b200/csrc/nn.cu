@@ -753,24 +753,6 @@ __global__ void __launch_bounds__(256, KMAX <= 20 ? 2 : 1) thin_dw_kernel(const 
     for (int i = threadIdx.x; i < N; i += blockDim.x) atomicAdd(db + i, sred[K * N + i]);
 }
 
-static int thin_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200RL_THIN");
-    v = e ? atoi(e) : 1;
-  }
-  return v;
-}
-
-static int skinny_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200RL_SKINNY");
-    v = e ? atoi(e) : 1;
-  }
-  return v;
-}
-
 // col2im in gather form (deterministic): dX[n,y,x,c] = sum over kernel taps hitting (y,x).
 __global__ void col2im_kernel(const float* __restrict__ dcol, float* __restrict__ dX, ConvGeom g,
                               int64_t total, int Kc, const ActMask mask) {
@@ -801,6 +783,38 @@ __global__ void col2im_kernel(const float* __restrict__ dcol, float* __restrict_
 // ---------------------------------------------------------------------------------------
 // host-side dispatch
 // ---------------------------------------------------------------------------------------
+// Dispatch settings, read from the environment once, on first use:
+//   B200RL_GEMM_MODE       0 = fp32 FFMA (sgemm_kernel), 1 = wgmma 3xTF32 (default),
+//                          2 = wgmma single-pass TF32 (not 1e-5 safe); b200rl_set_gemm_mode overrides it
+//   B200RL_THIN / B200RL_SKINNY / B200RL_FUSE_BIAS_GRAD   default 1; 0 turns off the thin-input
+//                          kernels / the skinny-head kernels / the bias gradient fused into the
+//                          tensor-core weight gradient (A/B switches for profiles/)
+struct Settings {
+  int gemm_mode, thin, skinny, fuse_bias_grad;
+};
+static int env_int(const char* name, int dflt) {
+  const char* e = getenv(name);
+  return e ? atoi(e) : dflt;
+}
+static Settings& settings() {
+  static Settings s{env_int("B200RL_GEMM_MODE", 1), env_int("B200RL_THIN", 1),
+                    env_int("B200RL_SKINNY", 1), env_int("B200RL_FUSE_BIAS_GRAD", 1)};
+  return s;
+}
+
+static bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+// Zeroes bytes at p on st; p == NULL (an optional gradient that is not wanted) is a no-op.
+static int zero_async(void* p, size_t bytes, cudaStream_t st, const char* what) {
+  if (p == nullptr) return B200RL_OK;
+  cudaError_t e = cudaMemsetAsync(p, 0, bytes, st);
+  if (e != cudaSuccess) {
+    set_error("%s: memset failed: %s", what, cudaGetErrorString(e));
+    return B200RL_ERR_CUDA;
+  }
+  return B200RL_OK;
+}
+
 struct GemmArgs {
   float* C;
   const float* bias;
@@ -811,57 +825,53 @@ struct GemmArgs {
   cudaStream_t st;
   float out_scale = 1.f;  // tensor-core path only: multiplies the accumulator (raw-u8 operands)
   ActMask mask{};         // input-gradient GEMMs: multiply the result by act'(mask.y)
+  // split-K partial slices of C that fit in the workspace (0 without one)
+  int64_t ws_slices() const { return ws ? ws_bytes / (M * N * (int64_t)sizeof(float)) : 0; }
 };
+
+// The smallest GEMM (in GEMM coordinates) the tensor-core kernels take.
+static bool tc_fits(int64_t M, int64_t N, int64_t K) { return N >= 16 && M >= 32 && K >= 8; }
+
+struct SplitK {
+  int splits;
+  int64_t kps;  // K range per split, a multiple of bk
+};
+// Split-K over grid.z when the tile grid leaves the chip short of `target` CTAs and K spans at
+// least 8 blocks of bk: ceil (round_up) or floor of target / tiles splits, each keeping at least
+// 4 blocks, at most max_splits and 65535.  The K range is then rounded up to whole blocks and the
+// splits recounted.
+static SplitK plan_split_k(int64_t tiles, int64_t K, int64_t bk, int64_t target, bool round_up,
+                           int64_t max_splits) {
+  int64_t s = 1;
+  if (tiles < target && K >= 8 * bk) {
+    s = round_up ? (target + tiles - 1) / tiles : target / tiles;
+    if (s > K / (4 * bk)) s = K / (4 * bk);
+    if (s > max_splits) s = max_splits;
+    if (s > 65535) s = 65535;
+    if (s < 2) s = 1;
+  }
+  int64_t kps = (K + s - 1) / s;
+  kps = (kps + bk - 1) / bk * bk;
+  return {(int)((K + kps - 1) / kps), kps};
+}
+
+static int splitk_reduce(const GemmArgs& g, int splits) {
+  const int64_t MN = g.M * g.N;
+  B200RL_LAUNCH(splitk_reduce_kernel, (unsigned)((MN + 255) / 256), 256, 0, g.st, (const float*)g.ws, g.C, g.bias, MN, g.N, splits, g.act, g.beta, g.mask);
+  B200RL_CHECK_LAUNCH("splitk_reduce");
+  return B200RL_OK;
+}
 
 template <int BM, int BN, int TM, int TN, class AL, class BL>
 static int launch_gemm_cfg(const AL& a, const BL& b, const GemmArgs& g) {
   const int64_t tm = (g.M + BM - 1) / BM, tn = (g.N + BN - 1) / BN;
-  const int64_t tiles = tm * tn;
-  int splits = 1;
-  const int64_t target = 2 * kNumSMs;
-  if (tiles < target && g.K >= 8 * BK && g.ws != nullptr) {
-    int64_t want = (target + tiles - 1) / tiles;
-    int64_t max_by_k = g.K / (4 * BK);
-    int64_t max_by_ws = g.ws_bytes / (int64_t)(g.M * g.N * sizeof(float));
-    int64_t s = want;
-    if (s > max_by_k) s = max_by_k;
-    if (s > max_by_ws) s = max_by_ws;
-    if (s > 65535) s = 65535;
-    if (s >= 2) splits = (int)s;
-  }
-  int64_t kps = (g.K + splits - 1) / splits;
-  kps = (kps + BK - 1) / BK * BK;
-  splits = (int)((g.K + kps - 1) / kps);
-  if (splits < 1) splits = 1;
+  // two CTAs per SM; the partials always go through the workspace
+  const SplitK sk = plan_split_k(tm * tn, g.K, BK, 2 * kNumSMs, true, g.ws_slices());
   B200RL_CHECK_ARG(tm <= 65535, "gemm: M too large for grid.y (%lld tiles)", (long long)tm);
-  dim3 grid((unsigned)tn, (unsigned)tm, (unsigned)splits);
-  B200RL_LAUNCH((sgemm_kernel<BM, BN, TM, TN, AL, BL>), grid, 256, 0, g.st, a, b, g.C, g.bias, g.M, g.N, g.K, g.act, g.beta, splits, kps, (float*)g.ws, g.mask);
+  dim3 grid((unsigned)tn, (unsigned)tm, (unsigned)sk.splits);
+  B200RL_LAUNCH((sgemm_kernel<BM, BN, TM, TN, AL, BL>), grid, 256, 0, g.st, a, b, g.C, g.bias, g.M, g.N, g.K, g.act, g.beta, sk.splits, sk.kps, (float*)g.ws, g.mask);
   B200RL_CHECK_LAUNCH("sgemm");
-  if (splits > 1) {
-    const int64_t MN = g.M * g.N;
-    B200RL_LAUNCH(splitk_reduce_kernel, (unsigned)((MN + 255) / 256), 256, 0, g.st, (const float*)g.ws, g.C, g.bias, MN, g.N, splits, g.act, g.beta, g.mask);
-    B200RL_CHECK_LAUNCH("splitk_reduce");
-  }
-  return B200RL_OK;
-}
-
-// 0 = fp32 FFMA (sgemm_kernel), 1 = wgmma 3xTF32, 2 = wgmma single-pass TF32 (not 1e-5 safe)
-// B200RL_FUSE_BIAS_GRAD=0 keeps the separate column-sum kernels (A/B switch for profiles/)
-static int fuse_bias_grad() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200RL_FUSE_BIAS_GRAD");
-    v = e ? atoi(e) : 1;
-  }
-  return v;
-}
-static int g_gemm_mode = -1;
-static int gemm_mode() {
-  if (g_gemm_mode < 0) {
-    const char* e = getenv("B200RL_GEMM_MODE");
-    g_gemm_mode = e ? atoi(e) : 1;
-  }
-  return g_gemm_mode;
+  return sk.splits > 1 ? splitk_reduce(g, sk.splits) : B200RL_OK;
 }
 
 template <int BN, int PASSES, int EPI, class AL, class BL>
@@ -882,68 +892,48 @@ static int launch_tc_cfg(const AL& a, const BL& b, const GemmArgs& g, const tc::
     configured = true;
   }
   const int64_t tm = (g.M + tc::kBM - 1) / tc::kBM, tn = (g.N + BN - 1) / BN;
-  const int64_t tiles = tm * tn;
-  int splits = 1;
-  const int64_t target = kNumSMs;  // resident CTAs on the chip (one per SM)
-  if (tiles < target && g.K >= 8 * tc::kBK && (g.ws != nullptr || EPI != tc::EPI_STORE)) {
-    int64_t want = target / tiles;  // only split when a whole extra set of CTAs fits on the chip
-    int64_t max_by_k = g.K / (4 * tc::kBK);
-    int64_t max_by_ws = EPI != tc::EPI_STORE ? 65535 : g.ws_bytes / (int64_t)(g.M * g.N * sizeof(float));
-    int64_t s = want < max_by_k ? want : max_by_k;
-    if (s > max_by_ws) s = max_by_ws;
-    if (s > 65535) s = 65535;
-    if (s >= 2) splits = (int)s;
-  }
-  int64_t kps = (g.K + splits - 1) / splits;
-  kps = (kps + tc::kBK - 1) / tc::kBK * tc::kBK;
-  splits = (int)((g.K + kps - 1) / kps);
-  if (splits < 1) splits = 1;
+  // one resident CTA per SM: only split when a whole extra set of CTAs fits on the chip.  The
+  // atomic and col2im epilogues add their partials in place; only EPI_STORE needs the workspace.
+  const SplitK sk = plan_split_k(tm * tn, g.K, tc::kBK, kNumSMs, false,
+                                 EPI == tc::EPI_STORE ? g.ws_slices() : 65535);
   B200RL_CHECK_ARG(tm <= 65535, "tc_gemm: M too large for grid.y (%lld tiles)", (long long)tm);
-  dim3 grid((unsigned)tn, (unsigned)tm, (unsigned)splits);
+  dim3 grid((unsigned)tn, (unsigned)tm, (unsigned)sk.splits);
   // a K range longer than one accumulation chain needs the chained variant to stay fp32-accurate
-  auto kernel = kps > tc::kChainBlocks * tc::kBK ? long_k : short_k;
-  B200RL_LAUNCH(kernel, grid, tc::kThreads, L::kBytes, g.st, a, b, epi, g.C, g.bias, g.M, g.N, g.K, g.act, g.beta, splits, kps, (float*)g.ws, g.out_scale);
+  auto kernel = sk.kps > tc::kChainBlocks * tc::kBK ? long_k : short_k;
+  B200RL_LAUNCH(kernel, grid, tc::kThreads, L::kBytes, g.st, a, b, epi, g.C, g.bias, g.M, g.N, g.K, g.act, g.beta, sk.splits, sk.kps, (float*)g.ws, g.out_scale);
   B200RL_CHECK_LAUNCH("tc_gemm");
-  if (splits > 1 && EPI == tc::EPI_STORE) {
-    const int64_t MN = g.M * g.N;
-    B200RL_LAUNCH(splitk_reduce_kernel, (unsigned)((MN + 255) / 256), 256, 0, g.st, (const float*)g.ws, g.C, g.bias, MN, g.N, splits, g.act, g.beta, g.mask);
-    B200RL_CHECK_LAUNCH("splitk_reduce");
-  }
-  return B200RL_OK;
+  return sk.splits > 1 && EPI == tc::EPI_STORE ? splitk_reduce(g, sk.splits) : B200RL_OK;
 }
 
-
-static bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
-
-template <int PASSES, class AL, class BL>
-static int launch_tc(const AL& a, const BL& b, const GemmArgs& g) {
-  tc::EpiArgs none{};
-  none.mask = g.mask;
+// Tensor-core GEMM with a fixed pass count: BN by output width (32 / 64 / 128; col2im always 128).
+template <int PASSES, int EPI, class AL, class BL>
+static int launch_tc_passes(const AL& a, const BL& b, const GemmArgs& g, const tc::EpiArgs& epi) {
   B200RL_CHECK_ARG(!(g.mask.y && g.beta), "gemm: an input-gradient mask cannot be combined with accumulation");
-  if (g.N <= 32) return launch_tc_cfg<32, PASSES, tc::EPI_STORE>(a, b, g, none);
-  if (g.N <= 64) return launch_tc_cfg<64, PASSES, tc::EPI_STORE>(a, b, g, none);
-  return launch_tc_cfg<128, PASSES, tc::EPI_STORE>(a, b, g, none);
+  if constexpr (EPI == tc::EPI_COL2IM) {
+    return launch_tc_cfg<128, PASSES, EPI>(a, b, g, epi);
+  } else {
+    if (g.N <= 32) return launch_tc_cfg<32, PASSES, EPI>(a, b, g, epi);
+    if (g.N <= 64) return launch_tc_cfg<64, PASSES, EPI>(a, b, g, epi);
+    return launch_tc_cfg<128, PASSES, EPI>(a, b, g, epi);
+  }
 }
 
-// Weight-gradient GEMMs (no bias / activation): in tensor-core mode the split-K partials are
-// accumulated with red.global.add straight into the (zeroed) gradient instead of going through
-// a workspace + reduce kernel.  Summation order across splits is not fixed.
-// `db` (optional): bias gradient = column sums of B; when the tensor-core path takes the GEMM and
-// B is an MN-major view the sums are accumulated by the producers of the same kernel and
-// *db_fused is set, otherwise the caller runs the separate column-sum kernels.
-template <class AL, class BL>
-static int launch_grad_gemm(const AL& a, const BL& b, const GemmArgs& g, float* db = nullptr,
-                            bool* db_fused = nullptr);
+// Tensor-core GEMM in the current mode: 2 = single-pass TF32, otherwise 3xTF32.
+template <int EPI, class AL, class BL>
+static int launch_tc(const AL& a, const BL& b, const GemmArgs& g, const tc::EpiArgs& epi) {
+  if (settings().gemm_mode == 2) return launch_tc_passes<1, EPI>(a, b, g, epi);
+  return launch_tc_passes<3, EPI>(a, b, g, epi);
+}
 
 template <class AL, class BL>
 static int launch_gemm(const AL& a, const BL& b, const GemmArgs& g) {
   if (g.M <= 0 || g.N <= 0) return B200RL_OK;
   B200RL_CHECK_ARG(g.K > 0, "gemm: K must be > 0");
   B200RL_CHECK_ARG(g.M < (1ll << 31) && g.N < (1ll << 31) && g.K < (1ll << 31), "gemm: dims");
-  const int mode = gemm_mode();
-  if (mode != 0 && g.N >= 16 && g.M >= 32 && g.K >= 8) {
-    if (mode == 2) return launch_tc<1>(a, b, g);
-    return launch_tc<3>(a, b, g);
+  if (settings().gemm_mode != 0 && tc_fits(g.M, g.N, g.K)) {
+    tc::EpiArgs epi{};
+    epi.mask = g.mask;
+    return launch_tc<tc::EPI_STORE>(a, b, g, epi);
   }
   if (g.N <= 32) return launch_gemm_cfg<128, 32, 4, 4>(a, b, g);
   if (g.N <= 64) {
@@ -955,41 +945,32 @@ static int launch_gemm(const AL& a, const BL& b, const GemmArgs& g) {
   return launch_gemm_cfg<64, 64, 4, 4>(a, b, g);
 }
 
+// Weight-gradient GEMMs (no bias / activation): in tensor-core mode the split-K partials are
+// accumulated with red.global.add straight into the (zeroed) gradient instead of going through
+// a workspace + reduce kernel.  Summation order across splits is not fixed.
+// `db` (optional): bias gradient = column sums of B; when the tensor-core path takes the GEMM and
+// B is an MN-major view the sums are accumulated by the producers of the same kernel and
+// *db_fused is set, otherwise the caller runs the separate column-sum kernels.
 template <class AL, class BL>
 static int launch_grad_gemm(const AL& a, const BL& b, const GemmArgs& g, float* db, bool* db_fused) {
-  const int mode = gemm_mode();
-  if (db_fused) *db_fused = false;
-  if (mode == 0 || g.N < 16 || g.M < 32 || g.K < 8 || g.bias != nullptr || g.act != B200RL_ACT_NONE)
-    return launch_gemm(a, b, g);
-  const bool fuse_db = db != nullptr && !BL::kKContig && fuse_bias_grad();
+  *db_fused = false;
+  if (settings().gemm_mode == 0 || !tc_fits(g.M, g.N, g.K)) return launch_gemm(a, b, g);
+  tc::EpiArgs epi{};
+  if (db != nullptr && !BL::kKContig && settings().fuse_bias_grad) epi.colsum = db;
   if (!g.beta) {
-    cudaError_t e = cudaMemsetAsync(g.C, 0, (size_t)(g.M * g.N) * sizeof(float), g.st);
-    if (e == cudaSuccess && fuse_db) e = cudaMemsetAsync(db, 0, (size_t)g.N * sizeof(float), g.st);
-    if (e != cudaSuccess) {
-      set_error("grad gemm: memset failed: %s", cudaGetErrorString(e));
-      return B200RL_ERR_CUDA;
-    }
+    int rc = zero_async(g.C, (size_t)(g.M * g.N) * sizeof(float), g.st, "grad gemm");
+    if (rc == B200RL_OK) rc = zero_async(epi.colsum, (size_t)g.N * sizeof(float), g.st, "grad gemm");
+    if (rc) return rc;
   }
-  tc::EpiArgs none{};
-  if (fuse_db) {
-    none.colsum = db;
-    if (db_fused) *db_fused = true;
-  }
-  if (mode == 2) {
-    if (g.N <= 32) return launch_tc_cfg<32, 1, tc::EPI_ATOMIC>(a, b, g, none);
-    if (g.N <= 64) return launch_tc_cfg<64, 1, tc::EPI_ATOMIC>(a, b, g, none);
-    return launch_tc_cfg<128, 1, tc::EPI_ATOMIC>(a, b, g, none);
-  }
-  if (g.N <= 32) return launch_tc_cfg<32, 3, tc::EPI_ATOMIC>(a, b, g, none);
-  if (g.N <= 64) return launch_tc_cfg<64, 3, tc::EPI_ATOMIC>(a, b, g, none);
-  return launch_tc_cfg<128, 3, tc::EPI_ATOMIC>(a, b, g, none);
+  *db_fused = epi.colsum != nullptr;
+  return launch_tc<tc::EPI_ATOMIC>(a, b, g, epi);
 }
 
 
 // ---- skinny-head dispatch (N <= 16) ----------------------------------------------------------
 static bool skinny_ok(int64_t M, int64_t K, int64_t N) {
-  return gemm_mode() != 0 && skinny_enabled() && N >= 1 && N <= kSkinnyMaxN && K >= 1 && K <= 1024 &&
-         K * N * (int64_t)sizeof(float) <= kSkinnySmem && M >= 1;
+  return settings().gemm_mode != 0 && settings().skinny && N >= 1 && N <= kSkinnyMaxN && K >= 1 &&
+         K <= 1024 && K * N * (int64_t)sizeof(float) <= kSkinnySmem && M >= 1;
 }
 template <int NMAX>
 static int skinny_fwd_launch(const float* X, int64_t ldx, const float* W, const float* bias,
@@ -1013,12 +994,9 @@ template <int NMAX>
 static int skinny_dw_launch(const float* X, int64_t ldx, const float* dY, float* dW, float* db,
                             int64_t M, int64_t K, int64_t N, int accumulate, cudaStream_t st) {
   if (!accumulate) {
-    cudaError_t e = cudaMemsetAsync(dW, 0, (size_t)(K * N) * sizeof(float), st);
-    if (e == cudaSuccess && db) e = cudaMemsetAsync(db, 0, (size_t)N * sizeof(float), st);
-    if (e != cudaSuccess) {
-      set_error("skinny dW: memset failed: %s", cudaGetErrorString(e));
-      return B200RL_ERR_CUDA;
-    }
+    int rc = zero_async(dW, (size_t)(K * N) * sizeof(float), st, "skinny dW");
+    if (rc == B200RL_OK) rc = zero_async(db, (size_t)N * sizeof(float), st, "skinny dW");
+    if (rc) return rc;
   }
   int64_t rows = (M + 2 * kNumSMs - 1) / (2 * kNumSMs);   // ~2 CTAs per SM; small M: 8-row slabs
   rows = (rows + 7) / 8 * 8;
@@ -1083,9 +1061,9 @@ int b200rl_tc_debug_buffer(long long* dev_buf) {
 }
 
 // ---- thin-input dispatch (K <= 32, 16 < N <= 256, N % 4 == 0) -----------------------------------
-static bool thin_ok(const float* X, int64_t ldx, const float* W, int64_t M, int64_t K, int64_t N) {
-  return gemm_mode() != 0 && thin_enabled() && K >= 1 && K <= kThinMaxK && N > kSkinnyMaxN &&
-         N <= kThinMaxN && (N & 3) == 0 && M >= 1 && al16(W);
+static bool thin_ok(const float* W, int64_t M, int64_t K, int64_t N) {
+  return settings().gemm_mode != 0 && settings().thin && K >= 1 && K <= kThinMaxK &&
+         N > kSkinnyMaxN && N <= kThinMaxN && (N & 3) == 0 && M >= 1 && al16(W);
 }
 static int thin_fwd_launch(const float* X, int64_t ldx, const float* W, const float* bias, float* Y,
                            int64_t M, int64_t K, int64_t N, int act, cudaStream_t st) {
@@ -1100,12 +1078,9 @@ static int thin_fwd_launch(const float* X, int64_t ldx, const float* W, const fl
 static int thin_dw_launch(const float* X, int64_t ldx, const float* dZ, float* dW, float* db,
                           int64_t M, int64_t K, int64_t N, int accumulate, cudaStream_t st) {
   if (!accumulate) {
-    cudaError_t e = cudaMemsetAsync(dW, 0, (size_t)(K * N) * sizeof(float), st);
-    if (e == cudaSuccess && db) e = cudaMemsetAsync(db, 0, (size_t)N * sizeof(float), st);
-    if (e != cudaSuccess) {
-      set_error("thin dW: memset failed: %s", cudaGetErrorString(e));
-      return B200RL_ERR_CUDA;
-    }
+    int rc = zero_async(dW, (size_t)(K * N) * sizeof(float), st, "thin dW");
+    if (rc == B200RL_OK) rc = zero_async(db, (size_t)N * sizeof(float), st, "thin dW");
+    if (rc) return rc;
   }
   int64_t rows = (M + 4 * kNumSMs - 1) / (4 * kNumSMs);
   rows = (rows + kThinRows - 1) / kThinRows * kThinRows;
@@ -1122,7 +1097,7 @@ static int thin_dw_launch(const float* X, int64_t ldx, const float* dZ, float* d
 int b200rl_set_gemm_mode(int mode) {
   B200RL_CHECK_ARG(mode >= 0 && mode <= 2, "gemm mode must be 0 (fp32 FFMA), 1 (wgmma 3xTF32) "
                                            "or 2 (wgmma 1xTF32)");
-  g_gemm_mode = mode;
+  settings().gemm_mode = mode;
   return B200RL_OK;
 }
 
@@ -1131,13 +1106,13 @@ int b200rl_dense_fwd(const float* X, int64_t ldx, const float* W, const float* b
                      int64_t ws_bytes, void* stream) {
   B200RL_CHECK_ARG(X && W && Y, "dense_fwd: NULL argument");
   B200RL_CHECK_ARG(ldx == 0 || ldx >= K, "dense_fwd: ldx < K");
-  if (skinny_ok(M, K, N))
-    return SKINNY_BY_N(skinny_fwd_launch, N, X, ldx ? ldx : K, W, bias, Y, M, K, N, act,
-                       (cudaStream_t)stream);
-  if (thin_ok(X, ldx, W, M, K, N) && al16(Y) && (bias == nullptr || al16(bias)))
-    return thin_fwd_launch(X, ldx ? ldx : K, W, bias, Y, M, K, N, act, (cudaStream_t)stream);
-  GemmArgs g{Y, bias, M, N, K, act, 0, workspace, ws_bytes, (cudaStream_t)stream};
-  return launch_gemm(ARow{X, ldx ? ldx : K}, BRow{W, N}, g);
+  if (ldx == 0) ldx = K;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (skinny_ok(M, K, N)) return SKINNY_BY_N(skinny_fwd_launch, N, X, ldx, W, bias, Y, M, K, N, act, st);
+  if (thin_ok(W, M, K, N) && al16(Y) && (bias == nullptr || al16(bias)))
+    return thin_fwd_launch(X, ldx, W, bias, Y, M, K, N, act, st);
+  GemmArgs g{Y, bias, M, N, K, act, 0, workspace, ws_bytes, st};
+  return launch_gemm(ARow{X, ldx}, BRow{W, N}, g);
 }
 
 int b200rl_dense_fwd_pair(const float* X1, const float* X2, int64_t ldx, const float* W1,
@@ -1146,16 +1121,9 @@ int b200rl_dense_fwd_pair(const float* X1, const float* X2, int64_t ldx, const f
                           int64_t ws_bytes, void* stream) {
   B200RL_CHECK_ARG(X1 && X2 && W1 && W2 && Y1 && Y2, "dense_fwd_pair: NULL argument");
   B200RL_CHECK_ARG(ldx == 0 || ldx >= K, "dense_fwd_pair: ldx < K");
-  if (skinny_ok(M, K, N) || (thin_ok(X1, ldx, W1, M, K, N) && thin_ok(X2, ldx, W2, M, K, N))) {
-    int rc = b200rl_dense_fwd(X1, ldx, W1, bias1, Y1, M, K, N, act, workspace, ws_bytes, stream);
-    if (rc) return rc;
-    return b200rl_dense_fwd(X2, ldx, W2, bias2, Y2, M, K, N, act, workspace, ws_bytes, stream);
-  }
-  GemmArgs g1{Y1, bias1, M, N, K, act, 0, workspace, ws_bytes, (cudaStream_t)stream};
-  GemmArgs g2{Y2, bias2, M, N, K, act, 0, workspace, ws_bytes, (cudaStream_t)stream};
-  int rc = launch_gemm(ARow{X1, ldx ? ldx : K}, BRow{W1, N}, g1);
+  int rc = b200rl_dense_fwd(X1, ldx, W1, bias1, Y1, M, K, N, act, workspace, ws_bytes, stream);
   if (rc) return rc;
-  return launch_gemm(ARow{X2, ldx ? ldx : K}, BRow{W2, N}, g2);
+  return b200rl_dense_fwd(X2, ldx, W2, bias2, Y2, M, K, N, act, workspace, ws_bytes, stream);
 }
 
 int b200rl_dense_bwd(const float* X, int64_t ldx, const float* W, const float* dY, float* dX,
@@ -1164,44 +1132,37 @@ int b200rl_dense_bwd(const float* X, int64_t ldx, const float* W, const float* d
   B200RL_CHECK_ARG(X && W && dY, "dense_bwd: NULL argument");
   B200RL_CHECK_ARG(ldx == 0 || ldx >= K, "dense_bwd: ldx < K");
   B200RL_CHECK_ARG(x_act >= B200RL_ACT_NONE && x_act <= B200RL_ACT_TANH, "dense_bwd: x_act");
+  if (ldx == 0) ldx = K;
   cudaStream_t st = (cudaStream_t)stream;
+  ActMask mask{};
+  if (x_act != B200RL_ACT_NONE) mask = ActMask{X, ldx, x_act};
   int rc;
   if (skinny_ok(M, K, N)) {
     if (dX) {
-      ActMask mask{};
-      if (x_act != B200RL_ACT_NONE) mask = ActMask{X, ldx ? ldx : K, x_act};
       rc = SKINNY_BY_N(skinny_dx_launch, N, dY, W, dX, M, K, N, mask, st);
       if (rc) return rc;
     }
-    if (dW) {
-      rc = SKINNY_BY_N(skinny_dw_launch, N, X, ldx ? ldx : K, dY, dW, db, M, K, N, accumulate, st);
-      if (rc) return rc;
-    } else if (db) {
-      rc = colsum(dY, db, M, N, accumulate, workspace, ws_bytes, st);
-      if (rc) return rc;
-    }
+    if (dW) return SKINNY_BY_N(skinny_dw_launch, N, X, ldx, dY, dW, db, M, K, N, accumulate, st);
+    if (db) return colsum(dY, db, M, N, accumulate, workspace, ws_bytes, st);
     return B200RL_OK;
   }
-  if (dX) {
+  if (dX) {  // dX[M,K] = dY @ W^T
     GemmArgs g{dX, nullptr, M, K, N, B200RL_ACT_NONE, 0, workspace, ws_bytes, st};
-    if (x_act != B200RL_ACT_NONE) g.mask = ActMask{X, ldx ? ldx : K, x_act};
+    g.mask = mask;
     rc = launch_gemm(ARow{dY, N}, BCol{W, N}, g);
     if (rc) return rc;
   }
   bool db_fused = false;
-  if (dW && thin_ok(X, ldx, W, M, K, N) && al16(dY)) {
-    rc = thin_dw_launch(X, ldx ? ldx : K, dY, dW, db, M, K, N, accumulate, st);
+  if (dW && thin_ok(W, M, K, N) && al16(dY)) {
+    rc = thin_dw_launch(X, ldx, dY, dW, db, M, K, N, accumulate, st);
     if (rc) return rc;
     db_fused = true;
-  } else if (dW) {
+  } else if (dW) {  // dW[K,N] = X^T @ dY
     GemmArgs g{dW, nullptr, K, N, M, B200RL_ACT_NONE, accumulate, workspace, ws_bytes, st};
-    rc = launch_grad_gemm(ACol{X, ldx ? ldx : K}, BRow{dY, N}, g, db, &db_fused);
+    rc = launch_grad_gemm(ACol{X, ldx}, BRow{dY, N}, g, db, &db_fused);
     if (rc) return rc;
   }
-  if (db && !db_fused) {
-    rc = colsum(dY, db, M, N, accumulate, workspace, ws_bytes, st);
-    if (rc) return rc;
-  }
+  if (db && !db_fused) return colsum(dY, db, M, N, accumulate, workspace, ws_bytes, st);
   return B200RL_OK;
 }
 
@@ -1226,17 +1187,15 @@ int b200rl_conv2d_fwd(const void* X, int x_is_u8, float x_scale, const float* Wt
   if (rc) return rc;
   const int64_t M = (int64_t)c->N * cg.OH * cg.OW, K = (int64_t)c->KH * c->KW * c->C;
   GemmArgs g{Y, bias, M, c->F, K, act, 0, workspace, ws_bytes, (cudaStream_t)stream};
-  if (x_is_u8) {
-    if (gemm_mode() == 1 && c->F >= 16 && M >= 32 && K >= 8) {   // raw pixels, 2-pass 3xTF32
-      g.out_scale = 1.f / x_scale;
-      AConvU8Raw a{ConvView<uint8_t>{(const uint8_t*)X, cg, x_scale}};
-      return launch_tc<3>(a, BRow{Wt, c->F}, g);
-    }
-    AConv<uint8_t> a{ConvView<uint8_t>{(const uint8_t*)X, cg, x_scale}};
-    return launch_gemm(a, BRow{Wt, c->F}, g);
+  const BRow w{Wt, c->F};
+  if (x_is_u8 && settings().gemm_mode == 1 && tc_fits(M, c->F, K)) {
+    // raw pixels, 2-pass 3xTF32, scaled in the epilogue (mode 1 only: no 1-pass kernels are built)
+    g.out_scale = 1.f / x_scale;
+    AConvU8Raw a{ConvView<uint8_t>{(const uint8_t*)X, cg, x_scale}};
+    return launch_tc_passes<3, tc::EPI_STORE>(a, w, g, tc::EpiArgs{});
   }
-  AConv<float> a{ConvView<float>{(const float*)X, cg, 1.f}};
-  return launch_gemm(a, BRow{Wt, c->F}, g);
+  if (x_is_u8) return launch_gemm(AConv<uint8_t>{ConvView<uint8_t>{(const uint8_t*)X, cg, x_scale}}, w, g);
+  return launch_gemm(AConv<float>{ConvView<float>{(const float*)X, cg, 1.f}}, w, g);
 }
 
 int b200rl_conv2d_fwd_pair(const void* X1, const void* X2, int x_is_u8, float x_scale,
@@ -1244,31 +1203,9 @@ int b200rl_conv2d_fwd_pair(const void* X1, const void* X2, int x_is_u8, float x_
                            const float* bias2, float* Y1, float* Y2, const b200rl_conv_t* c,
                            int act, void* workspace, int64_t ws_bytes, void* stream) {
   B200RL_CHECK_ARG(X1 && X2 && Wt1 && Wt2 && Y1 && Y2, "conv2d_fwd_pair: NULL argument");
-  ConvGeom cg;
-  int rc = make_geom(c, cg);
+  int rc = b200rl_conv2d_fwd(X1, x_is_u8, x_scale, Wt1, bias1, Y1, c, act, workspace, ws_bytes, stream);
   if (rc) return rc;
-  const int64_t M = (int64_t)c->N * cg.OH * cg.OW, K = (int64_t)c->KH * c->KW * c->C;
-  GemmArgs g1{Y1, bias1, M, c->F, K, act, 0, workspace, ws_bytes, (cudaStream_t)stream};
-  GemmArgs g2{Y2, bias2, M, c->F, K, act, 0, workspace, ws_bytes, (cudaStream_t)stream};
-  if (x_is_u8) {
-    if (gemm_mode() == 1 && c->F >= 16 && M >= 32 && K >= 8) {   // raw pixels, 2-pass 3xTF32
-      g1.out_scale = g2.out_scale = 1.f / x_scale;
-      AConvU8Raw a1{ConvView<uint8_t>{(const uint8_t*)X1, cg, x_scale}};
-      AConvU8Raw a2{ConvView<uint8_t>{(const uint8_t*)X2, cg, x_scale}};
-      const BRow b1{Wt1, c->F}, b2{Wt2, c->F};
-      rc = launch_tc<3>(a1, b1, g1);
-      if (rc) return rc;
-      return launch_tc<3>(a2, b2, g2);
-    }
-    rc = b200rl_conv2d_fwd(X1, x_is_u8, x_scale, Wt1, bias1, Y1, c, act, workspace, ws_bytes, stream);
-    if (rc) return rc;
-    return b200rl_conv2d_fwd(X2, x_is_u8, x_scale, Wt2, bias2, Y2, c, act, workspace, ws_bytes, stream);
-  }
-  AConv<float> a1{ConvView<float>{(const float*)X1, cg, 1.f}};
-  AConv<float> a2{ConvView<float>{(const float*)X2, cg, 1.f}};
-  rc = launch_gemm(a1, BRow{Wt1, c->F}, g1);
-  if (rc) return rc;
-  return launch_gemm(a2, BRow{Wt2, c->F}, g2);
+  return b200rl_conv2d_fwd(X2, x_is_u8, x_scale, Wt2, bias2, Y2, c, act, workspace, ws_bytes, stream);
 }
 
 int b200rl_conv2d_bwd(const void* X, int x_is_u8, float x_scale, const float* Wt,
@@ -1284,21 +1221,23 @@ int b200rl_conv2d_bwd(const void* X, int x_is_u8, float x_scale, const float* Wt
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t M = (int64_t)c->N * cg.OH * cg.OW, K = (int64_t)c->KH * c->KW * c->C;
   const int64_t F = c->F;
+  const int mode = settings().gemm_mode;
   ActMask mask{};
   if (x_act != B200RL_ACT_NONE && !x_is_u8) mask = ActMask{(const float*)X, cg.in_img, x_act};
   bool db_fused = false;
   if (dW) {  // dW[K,F] = im2col(X)^T @ dY
     GemmArgs g{dW, nullptr, K, F, M, B200RL_ACT_NONE, accumulate, workspace, ws_bytes, st};
-    if (x_is_u8 && gemm_mode() == 1 && F >= 16 && K >= 32 && M >= 8) {
+    const BRow dy{dY, F};
+    if (!x_is_u8) {
+      AConvT<float> a{ConvView<float>{(const float*)X, cg, 1.f}};
+      rc = launch_grad_gemm(a, dy, g, db, &db_fused);
+    } else if (mode == 1 && tc_fits(K, F, M)) {   // raw pixels, scaled in the epilogue
       g.out_scale = 1.f / x_scale;
       AConvTU8Raw a{ConvView<uint8_t>{(const uint8_t*)X, cg, x_scale}};
-      rc = launch_grad_gemm(a, BRow{dY, F}, g, db, &db_fused);
-    } else if (x_is_u8) {
+      rc = launch_grad_gemm(a, dy, g, db, &db_fused);
+    } else {  // mode 0 / 2: the STORE epilogue, bias gradient by the column-sum kernels
       AConvT<uint8_t> a{ConvView<uint8_t>{(const uint8_t*)X, cg, x_scale}};
-      rc = launch_gemm(a, BRow{dY, F}, g);
-    } else {
-      AConvT<float> a{ConvView<float>{(const float*)X, cg, 1.f}};
-      rc = launch_grad_gemm(a, BRow{dY, F}, g, db, &db_fused);
+      rc = launch_gemm(a, dy, g);
     }
     if (rc) return rc;
   }
@@ -1306,34 +1245,26 @@ int b200rl_conv2d_bwd(const void* X, int x_is_u8, float x_scale, const float* Wt
     rc = colsum(dY, db, M, F, accumulate, workspace, ws_bytes, st);
     if (rc) return rc;
   }
-  if (dX && gemm_mode() != 0 && (c->C & 3) == 0 && K >= 16 && M >= 32 && F >= 8) {
+  if (!dX) return B200RL_OK;
+  const int64_t total = (int64_t)c->N * c->H * c->W * c->C;
+  if (mode != 0 && (c->C & 3) == 0 && tc_fits(M, K, F)) {
     // tensor-core path: dY @ W^T with the col2im scatter-add fused into the epilogue
-    const int64_t total = (int64_t)c->N * c->H * c->W * c->C;
-    cudaError_t e = cudaMemsetAsync(dX, 0, (size_t)total * sizeof(float), st);
-    if (e != cudaSuccess) {
-      set_error("conv2d_bwd: memset failed: %s", cudaGetErrorString(e));
-      return B200RL_ERR_CUDA;
-    }
+    rc = zero_async(dX, (size_t)total * sizeof(float), st, "conv2d_bwd");
+    if (rc) return rc;
     GemmArgs g{nullptr, nullptr, M, K, F, B200RL_ACT_NONE, 0, nullptr, 0, st};
     tc::EpiArgs epi{cg, dX};
     epi.mask = mask;
-    const ARow da{dY, F};
-    const BCol db_{Wt, F};
-    if (gemm_mode() == 2) rc = launch_tc_cfg<128, 1, tc::EPI_COL2IM>(da, db_, g, epi);
-    else rc = launch_tc_cfg<128, 3, tc::EPI_COL2IM>(da, db_, g, epi);
-    if (rc) return rc;
-  } else if (dX) {  // dcol[M,K] = dY @ W^T, then gather-form col2im
-    const int64_t need = M * K * (int64_t)sizeof(float);
-    B200RL_CHECK_ARG(workspace && ws_bytes >= need,
-                     "conv2d_bwd: input gradient needs %lld bytes of workspace",
-                     (long long)need);
-    GemmArgs g{(float*)workspace, nullptr, M, K, F, B200RL_ACT_NONE, 0, nullptr, 0, st};
-    rc = launch_gemm(ARow{dY, F}, BCol{Wt, F}, g);
-    if (rc) return rc;
-    const int64_t total = (int64_t)c->N * c->H * c->W * c->C;
-    B200RL_LAUNCH(col2im_kernel, (unsigned)((total + 255) / 256), 256, 0, st, (const float*)workspace, dX, cg, total, (int)K, mask);
-    B200RL_CHECK_LAUNCH("col2im");
+    return launch_tc<tc::EPI_COL2IM>(ARow{dY, F}, BCol{Wt, F}, g, epi);
   }
+  // dcol[M,K] = dY @ W^T, then gather-form col2im
+  const int64_t need = M * K * (int64_t)sizeof(float);
+  B200RL_CHECK_ARG(workspace && ws_bytes >= need,
+                   "conv2d_bwd: input gradient needs %lld bytes of workspace", (long long)need);
+  GemmArgs g{(float*)workspace, nullptr, M, K, F, B200RL_ACT_NONE, 0, nullptr, 0, st};
+  rc = launch_gemm(ARow{dY, F}, BCol{Wt, F}, g);
+  if (rc) return rc;
+  B200RL_LAUNCH(col2im_kernel, (unsigned)((total + 255) / 256), 256, 0, st, (const float*)workspace, dX, cg, total, (int)K, mask);
+  B200RL_CHECK_LAUNCH("col2im");
   return B200RL_OK;
 }
 

@@ -497,7 +497,8 @@ int b200rl_cql_bc_actor_bwd(const float* head, const float* action, int64_t ld_a
  * 1 = Hopper wgmma tensor cores with the 3xTF32 split (fp32-grade accuracy, fp32 accumulators),
  * 2 = wgmma single-pass TF32 (~1e-3 relative; NOT within the 1e-5 parity bar).
  * Default: env B200RL_GEMM_MODE, else 1.  Outputs narrower than 16 columns (Q head, value head)
- * always use mode 0. */
+ * take the skinny-head kernels in modes 1 and 2, and the FFMA kernel in mode 0 or beyond the
+ * skinny limits (K > 1024, or K*N*4 bytes of weights over 48 KiB). */
 int b200rl_set_gemm_mode(int mode);
 /* Profiling aid: device buffer of int64[64][8] that receives %globaltimer phase stamps of the
  * first 64 CTAs of every tensor-core GEMM launch (NULL disables). */
@@ -510,8 +511,8 @@ int b200rl_dense_fwd(const float* X, int64_t ldx, const float* W, const float* b
                      int64_t M, int64_t K, int64_t N, int act, void* workspace,
                      int64_t ws_bytes, void* stream);
 /* Two dense layers of identical shape (X1 @ W1 + b1 -> Y1, X2 @ W2 + b2 -> Y2; biases both given
- * or both NULL) in one call: the same GEMM route as b200rl_dense_fwd, launched once per layer
- * (two launches, plus a split-K reduce each when the shape splits).  DqnAgent evaluates the
+ * or both NULL) in one call: b200rl_dense_fwd on each layer in turn, so each layer takes its own
+ * route (two launches, plus a split-K reduce each when the shape splits).  DqnAgent evaluates the
  * online network on obs[:, 0] and the target network on obs[:, T-1] this way
  * (agents/dqn/dqn_agent.py:488-520, :575-579 in the reference are the two independent forward
  * passes).  Workspace as b200rl_dense_fwd; the two launches use it one after the other. */
@@ -545,7 +546,7 @@ typedef struct {
 int b200rl_conv2d_fwd(const void* X, int x_is_u8, float x_scale, const float* Wt,
                       const float* bias, float* Y, const b200rl_conv_t* g, int act,
                       void* workspace, int64_t ws_bytes, void* stream);
-/* Two convolutions of identical geometry in one call, launched once per convolution (see
+/* Two convolutions of identical geometry in one call: b200rl_conv2d_fwd on each in turn (see
  * b200rl_dense_fwd_pair). */
 int b200rl_conv2d_fwd_pair(const void* X1, const void* X2, int x_is_u8, float x_scale,
                            const float* Wt1, const float* Wt2, const float* bias1,
