@@ -62,8 +62,6 @@ class B200RLError(RuntimeError):
 # name -> argtypes (restype is int unless listed in _RESTYPES)
 _P = c_void_p
 SIGNATURES = {
-    'b200rl_set_copy_variant': [c_int],
-    'b200rl_set_pdl': [c_int],
     'b200rl_rb_add_batch': [ctypes.POINTER(Ring), _P, _P],
     'b200rl_rb_sample': [ctypes.POINTER(Ring), c_i64, c_i64, _P, _P, c_u64, _P, _P, _P, _P, _P,
                          _P, _P],
@@ -126,10 +124,6 @@ SIGNATURES = {
     'b200rl_set_gemm_mode': [c_int],
     'b200rl_tc_debug_buffer': [_P],
     'b200rl_dense_fwd': [_P, c_i64, _P, _P, _P, c_i64, c_i64, c_i64, c_int, _P, c_i64, _P],
-    'b200rl_dense_fwd_pair': [_P, _P, c_i64, _P, _P, _P, _P, _P, _P, c_i64, c_i64, c_i64, c_int, _P,
-                              c_i64, _P],
-    'b200rl_conv2d_fwd_pair': [_P, _P, c_int, c_f32, _P, _P, _P, _P, _P, _P,
-                               ctypes.POINTER(ConvGeom), c_int, _P, c_i64, _P],
     'b200rl_dense_bwd': [_P, c_i64, _P, _P, _P, _P, _P, c_i64, c_i64, c_i64, c_int, c_int, _P, c_i64,
                          _P],
     'b200rl_act_bwd': [_P, _P, _P, c_i64, c_int, _P],
@@ -156,7 +150,6 @@ _RESTYPES = {
     'b200rl_last_error': ctypes.c_char_p,
     'b200rl_version': c_int,
     'b200rl_launch_count': c_i64,
-    'b200rl_get_pdl': c_int,
 }
 
 _lib = None

@@ -16,8 +16,6 @@ both evaluations are identical, so it is evaluated once here.
 """
 import collections
 
-import os
-
 import torch
 
 from agents_b200 import _lib
@@ -55,6 +53,9 @@ class DqnAgent(tf_agent.TFAgent):
   _DOUBLE_Q = False          # select the bootstrap action with the online network
   _SELECT_UNMASKED = False   # D3qn: raw argmax over the selector's output (no action constraints)
   _FUSED_TD_LOSS = True      # False: td_errors_loss_fn is accepted but not used (CategoricalDqnAgent)
+  # data-parallel runs all-reduce the gradient in buckets of at least this many bytes, overlapped
+  # with the rest of the backward pass
+  _bucket_bytes = 1 << 20
 
   def __init__(self, time_step_spec, action_spec, q_network, optimizer,
                observation_and_action_constraint_splitter=None, epsilon_greedy=0.1,
@@ -109,20 +110,10 @@ class DqnAgent(tf_agent.TFAgent):
         train_step_counter=train_step_counter, training_data_spec=training_data_spec,
         device=device)
     self._nan_flag = torch.zeros(1, dtype=torch.int32, device=device)
-    # 0 = never, 1 = inside common.function graphs (default), 2 = always
-    self._overlap_target = int(os.environ.get('B200RL_DQN_OVERLAP', '1'))
-    self._side_stream = torch.cuda.Stream(device=device) if self._overlap_target else None
-    # B200RL_DQN_PAIR_FWD=1: online + target forward as paired launches (Network.forward_pair).
-    # Off by default: measured SLOWER than the two-stream fork below (run 19: 2806 vs 2890
-    # steps/s, 25 vs 29 launches per step) -- with the target pass on its own stream the fill and
-    # drain of one network's kernels hide behind the other's, which the single paired launch loses.
-    self._pair_forward = int(os.environ.get('B200RL_DQN_PAIR_FWD', '0'))
+    self._side_stream = torch.cuda.Stream(device=device)
     self._clip_offsets = None
     self.replicas = 1           # set by train.Learner for data-parallel runs
     self._grad_sync = None      # callable(flat_grads) installed by train.Learner
-    # gradient all-reduce in buckets of at least this many bytes, overlapped with the rest of the
-    # backward pass (0: one all-reduce after the backward pass)
-    self._bucket_bytes = int(os.environ.get('B200RL_GRAD_BUCKET_BYTES', str(1 << 20)))
     self._comm_stream = torch.cuda.Stream(device=device)
 
   # ---- construction helpers -----------------------------------------------------------------
@@ -181,24 +172,11 @@ class DqnAgent(tf_agent.TFAgent):
     B, T = exp.discount.shape[0], exp.discount.shape[1]
     obs0, _ = self._split_obs(nest.map_structure(lambda t: t[:, 0], exp.observation))
     obsn, next_mask = self._split_obs(nest.map_structure(lambda t: t[:, T - 1], exp.observation))
-    # The target-side forwards do not depend on the online forward: fork them onto a side
-    # stream (also inside a captured graph) and join before the TD kernel.
+    # The target-side forwards do not depend on the online forward: inside a captured graph fork
+    # them onto a side stream and join before the TD kernel (eager launches are host-bound, the
+    # fork only pays inside a graph).
     main = torch.cuda.current_stream()
-    side = None
-    # Plain DQN: the online forward on obs[:, 0] and the target forward on obs[:, T-1] are two
-    # passes through identical layer stacks -> every layer pair is one launch.
-    if (self._pair_forward and not self._DOUBLE_Q and keep_tape and
-        self._q_network.pairs_with(self._target_q_network) and
-        hasattr(self._q_network, 'forward_pair')):
-      (q, tape), next_t = self._q_network.forward_pair(self._target_q_network, obs0, obsn)
-      if not isinstance(q, tuple) and not isinstance(next_t, tuple):
-        if self._SELECT_UNMASKED:
-          next_mask = None
-        return self._td(exp, B, T, q, next_t, next_t, next_mask, weights, tape)
-    if self._overlap_target == 2 or (self._overlap_target and
-                                     torch.cuda.is_current_stream_capturing()):
-      # eager launches are host-bound, the fork only pays inside a captured graph
-      side = self._side_stream
+    side = self._side_stream if torch.cuda.is_current_stream_capturing() else None
     if side is not None:
       side.wait_stream(main)
     with torch.cuda.stream(side if side is not None else main), \
@@ -219,13 +197,7 @@ class DqnAgent(tf_agent.TFAgent):
       (q, _), tape = self._q_network(obs0), None
     if side is not None:
       main.wait_stream(side)
-      if not torch.cuda.is_current_stream_capturing():
-        # eager fork (B200RL_DQN_OVERLAP=2): these tensors were allocated on the side stream and
-        # are consumed on the main one; tell the caching allocator before they can be recycled
-        next_t.record_stream(main)
-        if next_sel is not next_t:
-          next_sel.record_stream(main)
-    elif self._overlap_target and not torch.cuda.is_current_stream_capturing():
+    else:
       workspace.mirror(q.device, 1)   # size the side-stream scratch for a later capture
     return self._td(exp, B, T, q, next_t, next_sel, next_mask, weights, tape)
 
@@ -283,7 +255,7 @@ class DqnAgent(tf_agent.TFAgent):
     # Data-parallel runs: start the all-reduce of the gradient tail (the fc layers come out of
     # the backward pass first and hold 95 % of the bytes of the Atari net) on a communication
     # stream as soon as it is complete, and reduce the small head after the last conv gradient.
-    bucketed = self._grad_sync is not None and self._bucket_bytes > 0 and not reg
+    bucketed = self._grad_sync is not None and not reg
     hook = None
     if bucketed:
       total = net.flat_grads.numel()

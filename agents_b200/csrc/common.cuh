@@ -51,9 +51,7 @@ __device__ __forceinline__ void pdl_prologue() {
   pdl_launch_dependents();
 }
 
-// 1 when launches carry cudaLaunchAttributeProgrammaticStreamSerialization (B200RL_PDL, b200rl_set_pdl)
-int pdl_enabled();
-
+// Every launch carries cudaLaunchAttributeProgrammaticStreamSerialization.
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
                             cudaStream_t st, Args&&... args) {
@@ -63,12 +61,10 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
-  if (pdl_enabled()) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-  }
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<Args&&>(args)...);
 }
 // Launch errors are picked up by the B200RL_CHECK_LAUNCH that follows every launch.

@@ -2,7 +2,6 @@
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 
 #include "common.cuh"
 
@@ -20,28 +19,13 @@ void set_error(const char* fmt, ...) {
 
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
-static int g_pdl = -1;
-int pdl_enabled() {
-  if (g_pdl < 0) {
-    const char* e = getenv("B200RL_PDL");
-    g_pdl = e ? (atoi(e) != 0) : 1;   // on by default (B200RL_PDL=0 switches it off)
-  }
-  return g_pdl;
-}
-
 }  // namespace b200rl
 
 extern "C" {
 
 const char* b200rl_last_error(void) { return b200rl::g_err; }
-int b200rl_version(void) { return 100; }
+int b200rl_version(void) { return 101; }
 int64_t b200rl_launch_count(void) { return b200rl::g_launches.load(); }
-
-int b200rl_set_pdl(int enabled) {
-  b200rl::g_pdl = enabled ? 1 : 0;
-  return B200RL_OK;
-}
-int b200rl_get_pdl(void) { return b200rl::pdl_enabled(); }
 
 // Emission order of a `tf.data` style shuffle(buffer) over a stream of n elements
 // (train/ppo_learner.py:236-238).  Host-side like the reference's input pipeline; the

@@ -783,23 +783,15 @@ __global__ void col2im_kernel(const float* __restrict__ dcol, float* __restrict_
 // ---------------------------------------------------------------------------------------
 // host-side dispatch
 // ---------------------------------------------------------------------------------------
-// Dispatch settings, read from the environment once, on first use:
-//   B200RL_GEMM_MODE       0 = fp32 FFMA (sgemm_kernel), 1 = wgmma 3xTF32 (default),
-//                          2 = wgmma single-pass TF32 (not 1e-5 safe); b200rl_set_gemm_mode overrides it
-//   B200RL_THIN / B200RL_SKINNY / B200RL_FUSE_BIAS_GRAD   default 1; 0 turns off the thin-input
-//                          kernels / the skinny-head kernels / the bias gradient fused into the
-//                          tensor-core weight gradient (A/B switches for profiles/)
-struct Settings {
-  int gemm_mode, thin, skinny, fuse_bias_grad;
-};
-static int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : dflt;
-}
-static Settings& settings() {
-  static Settings s{env_int("B200RL_GEMM_MODE", 1), env_int("B200RL_THIN", 1),
-                    env_int("B200RL_SKINNY", 1), env_int("B200RL_FUSE_BIAS_GRAD", 1)};
-  return s;
+// GEMM mode, read from B200RL_GEMM_MODE once, on first use; b200rl_set_gemm_mode overrides it.
+//   0 = fp32 FFMA (sgemm_kernel), 1 = wgmma 3xTF32 (default),
+//   2 = wgmma single-pass TF32 (not 1e-5 safe)
+static int& gemm_mode() {
+  static int mode = [] {
+    const char* e = getenv("B200RL_GEMM_MODE");
+    return e ? atoi(e) : 1;
+  }();
+  return mode;
 }
 
 static bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
@@ -921,7 +913,7 @@ static int launch_tc_passes(const AL& a, const BL& b, const GemmArgs& g, const t
 // Tensor-core GEMM in the current mode: 2 = single-pass TF32, otherwise 3xTF32.
 template <int EPI, class AL, class BL>
 static int launch_tc(const AL& a, const BL& b, const GemmArgs& g, const tc::EpiArgs& epi) {
-  if (settings().gemm_mode == 2) return launch_tc_passes<1, EPI>(a, b, g, epi);
+  if (gemm_mode() == 2) return launch_tc_passes<1, EPI>(a, b, g, epi);
   return launch_tc_passes<3, EPI>(a, b, g, epi);
 }
 
@@ -930,7 +922,7 @@ static int launch_gemm(const AL& a, const BL& b, const GemmArgs& g) {
   if (g.M <= 0 || g.N <= 0) return B200RL_OK;
   B200RL_CHECK_ARG(g.K > 0, "gemm: K must be > 0");
   B200RL_CHECK_ARG(g.M < (1ll << 31) && g.N < (1ll << 31) && g.K < (1ll << 31), "gemm: dims");
-  if (settings().gemm_mode != 0 && tc_fits(g.M, g.N, g.K)) {
+  if (gemm_mode() != 0 && tc_fits(g.M, g.N, g.K)) {
     tc::EpiArgs epi{};
     epi.mask = g.mask;
     return launch_tc<tc::EPI_STORE>(a, b, g, epi);
@@ -954,9 +946,9 @@ static int launch_gemm(const AL& a, const BL& b, const GemmArgs& g) {
 template <class AL, class BL>
 static int launch_grad_gemm(const AL& a, const BL& b, const GemmArgs& g, float* db, bool* db_fused) {
   *db_fused = false;
-  if (settings().gemm_mode == 0 || !tc_fits(g.M, g.N, g.K)) return launch_gemm(a, b, g);
+  if (gemm_mode() == 0 || !tc_fits(g.M, g.N, g.K)) return launch_gemm(a, b, g);
   tc::EpiArgs epi{};
-  if (db != nullptr && !BL::kKContig && settings().fuse_bias_grad) epi.colsum = db;
+  if (db != nullptr && !BL::kKContig) epi.colsum = db;
   if (!g.beta) {
     int rc = zero_async(g.C, (size_t)(g.M * g.N) * sizeof(float), g.st, "grad gemm");
     if (rc == B200RL_OK) rc = zero_async(epi.colsum, (size_t)g.N * sizeof(float), g.st, "grad gemm");
@@ -969,8 +961,8 @@ static int launch_grad_gemm(const AL& a, const BL& b, const GemmArgs& g, float* 
 
 // ---- skinny-head dispatch (N <= 16) ----------------------------------------------------------
 static bool skinny_ok(int64_t M, int64_t K, int64_t N) {
-  return settings().gemm_mode != 0 && settings().skinny && N >= 1 && N <= kSkinnyMaxN && K >= 1 &&
-         K <= 1024 && K * N * (int64_t)sizeof(float) <= kSkinnySmem && M >= 1;
+  return gemm_mode() != 0 && N >= 1 && N <= kSkinnyMaxN && K >= 1 && K <= 1024 &&
+         K * N * (int64_t)sizeof(float) <= kSkinnySmem && M >= 1;
 }
 template <int NMAX>
 static int skinny_fwd_launch(const float* X, int64_t ldx, const float* W, const float* bias,
@@ -1062,8 +1054,8 @@ int b200rl_tc_debug_buffer(long long* dev_buf) {
 
 // ---- thin-input dispatch (K <= 32, 16 < N <= 256, N % 4 == 0) -----------------------------------
 static bool thin_ok(const float* W, int64_t M, int64_t K, int64_t N) {
-  return settings().gemm_mode != 0 && settings().thin && K >= 1 && K <= kThinMaxK &&
-         N > kSkinnyMaxN && N <= kThinMaxN && (N & 3) == 0 && M >= 1 && al16(W);
+  return gemm_mode() != 0 && K >= 1 && K <= kThinMaxK && N > kSkinnyMaxN && N <= kThinMaxN &&
+         (N & 3) == 0 && M >= 1 && al16(W);
 }
 static int thin_fwd_launch(const float* X, int64_t ldx, const float* W, const float* bias, float* Y,
                            int64_t M, int64_t K, int64_t N, int act, cudaStream_t st) {
@@ -1097,7 +1089,7 @@ static int thin_dw_launch(const float* X, int64_t ldx, const float* dZ, float* d
 int b200rl_set_gemm_mode(int mode) {
   B200RL_CHECK_ARG(mode >= 0 && mode <= 2, "gemm mode must be 0 (fp32 FFMA), 1 (wgmma 3xTF32) "
                                            "or 2 (wgmma 1xTF32)");
-  settings().gemm_mode = mode;
+  gemm_mode() = mode;
   return B200RL_OK;
 }
 
@@ -1113,17 +1105,6 @@ int b200rl_dense_fwd(const float* X, int64_t ldx, const float* W, const float* b
     return thin_fwd_launch(X, ldx, W, bias, Y, M, K, N, act, st);
   GemmArgs g{Y, bias, M, N, K, act, 0, workspace, ws_bytes, st};
   return launch_gemm(ARow{X, ldx}, BRow{W, N}, g);
-}
-
-int b200rl_dense_fwd_pair(const float* X1, const float* X2, int64_t ldx, const float* W1,
-                          const float* W2, const float* bias1, const float* bias2, float* Y1,
-                          float* Y2, int64_t M, int64_t K, int64_t N, int act, void* workspace,
-                          int64_t ws_bytes, void* stream) {
-  B200RL_CHECK_ARG(X1 && X2 && W1 && W2 && Y1 && Y2, "dense_fwd_pair: NULL argument");
-  B200RL_CHECK_ARG(ldx == 0 || ldx >= K, "dense_fwd_pair: ldx < K");
-  int rc = b200rl_dense_fwd(X1, ldx, W1, bias1, Y1, M, K, N, act, workspace, ws_bytes, stream);
-  if (rc) return rc;
-  return b200rl_dense_fwd(X2, ldx, W2, bias2, Y2, M, K, N, act, workspace, ws_bytes, stream);
 }
 
 int b200rl_dense_bwd(const float* X, int64_t ldx, const float* W, const float* dY, float* dX,
@@ -1188,7 +1169,7 @@ int b200rl_conv2d_fwd(const void* X, int x_is_u8, float x_scale, const float* Wt
   const int64_t M = (int64_t)c->N * cg.OH * cg.OW, K = (int64_t)c->KH * c->KW * c->C;
   GemmArgs g{Y, bias, M, c->F, K, act, 0, workspace, ws_bytes, (cudaStream_t)stream};
   const BRow w{Wt, c->F};
-  if (x_is_u8 && settings().gemm_mode == 1 && tc_fits(M, c->F, K)) {
+  if (x_is_u8 && gemm_mode() == 1 && tc_fits(M, c->F, K)) {
     // raw pixels, 2-pass 3xTF32, scaled in the epilogue (mode 1 only: no 1-pass kernels are built)
     g.out_scale = 1.f / x_scale;
     AConvU8Raw a{ConvView<uint8_t>{(const uint8_t*)X, cg, x_scale}};
@@ -1196,16 +1177,6 @@ int b200rl_conv2d_fwd(const void* X, int x_is_u8, float x_scale, const float* Wt
   }
   if (x_is_u8) return launch_gemm(AConv<uint8_t>{ConvView<uint8_t>{(const uint8_t*)X, cg, x_scale}}, w, g);
   return launch_gemm(AConv<float>{ConvView<float>{(const float*)X, cg, 1.f}}, w, g);
-}
-
-int b200rl_conv2d_fwd_pair(const void* X1, const void* X2, int x_is_u8, float x_scale,
-                           const float* Wt1, const float* Wt2, const float* bias1,
-                           const float* bias2, float* Y1, float* Y2, const b200rl_conv_t* c,
-                           int act, void* workspace, int64_t ws_bytes, void* stream) {
-  B200RL_CHECK_ARG(X1 && X2 && Wt1 && Wt2 && Y1 && Y2, "conv2d_fwd_pair: NULL argument");
-  int rc = b200rl_conv2d_fwd(X1, x_is_u8, x_scale, Wt1, bias1, Y1, c, act, workspace, ws_bytes, stream);
-  if (rc) return rc;
-  return b200rl_conv2d_fwd(X2, x_is_u8, x_scale, Wt2, bias2, Y2, c, act, workspace, ws_bytes, stream);
 }
 
 int b200rl_conv2d_bwd(const void* X, int x_is_u8, float x_scale, const float* Wt,
@@ -1221,7 +1192,7 @@ int b200rl_conv2d_bwd(const void* X, int x_is_u8, float x_scale, const float* Wt
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t M = (int64_t)c->N * cg.OH * cg.OW, K = (int64_t)c->KH * c->KW * c->C;
   const int64_t F = c->F;
-  const int mode = settings().gemm_mode;
+  const int mode = gemm_mode();
   ActMask mask{};
   if (x_act != B200RL_ACT_NONE && !x_is_u8) mask = ActMask{(const float*)X, cg.in_img, x_act};
   bool db_fused = false;

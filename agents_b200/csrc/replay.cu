@@ -344,17 +344,6 @@ __global__ void draw_kernel(const __grid_constant__ Plan p) {
 __global__ void clear_kernel(int64_t* last_id) {
   pdl_prologue(); *last_id = -1; }
 
-// 0 = LDG/STG kernel (row_copy_big), 1 = TMA bulk-copy kernel (row_copy_tma).
-// B200RL_COPY_VARIANT overrides the default (used by profiles/gather_sweep.py for A/B runs).
-static int g_copy_variant = -1;
-static int copy_variant() {
-  if (g_copy_variant < 0) {
-    const char* e = getenv("B200RL_COPY_VARIANT");
-    g_copy_variant = e ? atoi(e) : 1;
-  }
-  return g_copy_variant;
-}
-
 static int widest_vec(int64_t row_bytes, const void* a, const void* b) {
   uintptr_t bits = (uintptr_t)row_bytes | (uintptr_t)a | (uintptr_t)b;
   if ((bits & 15) == 0) return 16;
@@ -412,7 +401,8 @@ static int launch_plan(Plan& p, cudaStream_t st, const char* name) {
   if (p.n_big > 0) {
     int64_t grid = p.n_rows * p.pieces_per_row;
     B200RL_CHECK_ARG(grid < (1ll << 31), "%s: grid too large", name);
-    bool tma_ok = copy_variant() == 1;
+    // the TMA bulk copy (row_copy_tma) needs every big leaf 16-byte aligned, else row_copy_big
+    bool tma_ok = true;
     int max_piece = 0;
     for (int i = 0; i < p.n_big; ++i) {
       if (p.big[i].vec != 16) tma_ok = false;
@@ -437,12 +427,6 @@ static int launch_plan(Plan& p, cudaStream_t st, const char* name) {
 using namespace b200rl;
 
 extern "C" {
-
-int b200rl_set_copy_variant(int v) {
-  B200RL_CHECK_ARG(v == 0 || v == 1, "copy variant must be 0 (LDG) or 1 (TMA bulk)");
-  g_copy_variant = v;
-  return B200RL_OK;
-}
 
 int b200rl_rb_add_batch(const b200rl_ring_t* ring, const void* const* items, void* stream) {
   Plan p;

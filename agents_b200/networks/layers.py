@@ -158,25 +158,6 @@ class Dense(Layer):
               self.units, self._act, _lib.ptr(ws), nb, _lib.stream())
     return y
 
-  def forward_pair(self, other, x, x_other):
-    """`self.forward(x)` and `other.forward(x_other)` (a layer of identical shape in another
-    network) in one launch when the tensor-core path takes the shape."""
-    x, ldx = _batch_strided(x, self.in_features)
-    x2, ldx2 = _batch_strided(x_other, self.in_features)
-    m = x.shape[0]
-    if (ldx2 != ldx or x2.shape[0] != m or other.in_features != self.in_features or
-        other.units != self.units or other._act != self._act or
-        (other.bias is None) != (self.bias is None)):
-      return self.forward(x), other.forward(x_other)
-    y = torch.empty((m, self.units), dtype=torch.float32, device=x.device)
-    y2 = torch.empty_like(y)
-    ws, nb = workspace.get(x.device)
-    _lib.call('b200rl_dense_fwd_pair', _lib.dptr(x), _lib.dptr(x2), ldx, _lib.ptr(self.kernel),
-              _lib.ptr(other.kernel), _lib.ptr(self.bias), _lib.ptr(other.bias), _lib.ptr(y),
-              _lib.ptr(y2), m, self.in_features, self.units, self._act, _lib.ptr(ws), nb,
-              _lib.stream())
-    return y, y2
-
   def backward_act(self, y, dy):
     """dLoss/d(pre-activation) from dLoss/d(output)."""
     dy = dy.contiguous()
@@ -278,29 +259,6 @@ class Conv2D(Layer):
               _lib.ptr(self.kernel), _lib.ptr(self.bias), _lib.ptr(y), ctypes.byref(g), self._act,
               _lib.ptr(ws), nb, _lib.stream())
     return y
-
-  def forward_pair(self, other, x, x_other):
-    """See Dense.forward_pair."""
-    x, bstride, is_u8 = self._input(x)
-    x2, bstride2, is_u82 = other._input(x_other)
-    same = (bstride2 == bstride and is_u82 == is_u8 and tuple(x2.shape) == tuple(x.shape) and
-            (other.kh, other.kw, other.c, other.filters, other.stride, other._act) ==
-            (self.kh, self.kw, self.c, self.filters, self.stride, self._act) and
-            (other.pre_divisor or 1.0) == (self.pre_divisor or 1.0) and
-            (other.bias is None) == (self.bias is None))
-    if not same:
-      return self.forward(x), other.forward(x_other)
-    g = self._geom(x)
-    g.x_batch_stride = bstride
-    y = torch.empty((x.shape[0], self.oh, self.ow, self.filters), dtype=torch.float32,
-                    device=x.device)
-    y2 = torch.empty_like(y)
-    ws, nb = workspace.get(x.device)
-    _lib.call('b200rl_conv2d_fwd_pair', _lib.dptr(x), _lib.dptr(x2), int(is_u8),
-              float(self.pre_divisor or 1.0), _lib.ptr(self.kernel), _lib.ptr(other.kernel),
-              _lib.ptr(self.bias), _lib.ptr(other.bias), _lib.ptr(y), _lib.ptr(y2), ctypes.byref(g),
-              self._act, _lib.ptr(ws), nb, _lib.stream())
-    return y, y2
 
   def backward_act(self, y, dy):
     dy = dy.contiguous()

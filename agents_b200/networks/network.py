@@ -6,7 +6,6 @@ returns `(output, network_state)` like the reference; `forward_train` additional
 the activations needed by `backward`.
 """
 import copy as _copy
-import os
 
 import numpy as np
 import torch
@@ -205,35 +204,6 @@ class Network(object):
     out, _ = self._run(observation, keep=False)
     return out, network_state
 
-  def pairs_with(self, other):
-    """True when `other` has this network's layer sequence (a target copy), so that
-    `forward_pair` can fuse the two forward passes layer by layer."""
-    if type(other) is not type(self) or not getattr(other, '_built', False) or not self._built:
-      return False
-    mine = [l for l in self._layers if not isinstance(l, layers_lib.CastScale)]
-    theirs = [l for l in other._layers if not isinstance(l, layers_lib.CastScale)]
-    return len(mine) == len(theirs) and all(type(a) is type(b) for a, b in zip(mine, theirs))
-
-  def forward_pair(self, other, observation, other_observation, keep=True):
-    """`self.forward_train(observation)` and `other(other_observation)` with every layer pair
-    issued as ONE launch where the kernels support it (DqnAgent: online network on obs[:, 0],
-    target network on obs[:, T-1]).  Returns ((out, tape), other_out)."""
-    self._require_built()
-    other._require_built()
-    tape = []
-    x, x2 = observation, other_observation
-    theirs = [l for l in other._layers if not isinstance(l, layers_lib.CastScale)]
-    mine = [l for l in self._layers if not isinstance(l, layers_lib.CastScale)]
-    for l, l2 in zip(mine, theirs):
-      if hasattr(l, 'forward_pair'):
-        y, y2 = l.forward_pair(l2, x, x2)
-      else:
-        y, y2 = l.forward(x), l2.forward(x2)
-      if keep:
-        tape.append((l, x, y))
-      x, x2 = y, y2
-    return (x, tape), x2
-
   def forward_train(self, observation):
     """Forward that records activations; returns (output, tape)."""
     return self._run(observation, keep=True)
@@ -254,7 +224,7 @@ class Network(object):
     # Inside a captured graph the parameter gradients (dW GEMM + fused bias column sums) of every
     # layer are forked onto a side stream: only the dX chain stays on the critical path.
     side = _side_stream(self._device) if (
-        _BWD_OVERLAP and need_param_grads and torch.cuda.is_current_stream_capturing()) else None
+        need_param_grads and torch.cuda.is_current_stream_capturing()) else None
     main = torch.cuda.current_stream() if side is not None else None
     # The flat gradient is zeroed ONCE and every layer accumulates into its views (split-K weight
     # gradients and the fused bias sums are red.global.add epilogues): one fill instead of one
@@ -284,8 +254,7 @@ class Network(object):
       # Dense consumers fold act'(x) into their dX epilogue (one coalesced read per output row);
       # for Conv2D consumers the col2im epilogue would need a scattered read per red.add, which
       # measured slower than the separate vectorised act_bwd pass (profiles/r2/README.md)
-      fuse = _FUSE_ACT_BWD == 2 or (_FUSE_ACT_BWD == 1 and isinstance(l, layers_lib.Dense))
-      x_act = producer_act(i) if need_dx and fuse else _ACT_NONE
+      x_act = producer_act(i) if need_dx and isinstance(l, layers_lib.Dense) else _ACT_NONE
       if side is not None:
         side.wait_stream(main)                   # dz (and everything before it) is ready
         dz.record_stream(side)
@@ -309,7 +278,7 @@ class Network(object):
       dy_is_preact = x_act != _ACT_NONE
     if side is not None:
       main.wait_stream(side)
-    elif _BWD_OVERLAP and not torch.cuda.is_current_stream_capturing():
+    elif not torch.cuda.is_current_stream_capturing():
       workspace.mirror(self._device, 1)          # size the side-stream scratch for a later capture
       _side_stream(self._device)
     if need_input_grad:
@@ -317,9 +286,6 @@ class Network(object):
     return self._grads
 
 
-_BWD_OVERLAP = os.environ.get('B200RL_BWD_OVERLAP', '1') != '0'
-# act'(x) of the producing layer folded into the consumer's dX epilogue (0: separate act_bwd pass)
-_FUSE_ACT_BWD = int(os.environ.get('B200RL_FUSE_ACT_BWD', '1'))   # 0 never, 1 Dense consumers, 2 all
 _ACT_NONE = 0
 _SIDE_STREAMS = {}
 

@@ -53,13 +53,10 @@ const char* b200rl_last_error(void);
 int b200rl_version(void);
 /* Number of kernels this library has launched since load (bench.py's gpu_launches). */
 int64_t b200rl_launch_count(void);
-/* Programmatic dependent launch: when enabled (the default; B200RL_PDL=0 in the environment or
- * b200rl_set_pdl(0) switches it off) every kernel
- * is launched with cudaLaunchAttributeProgrammaticStreamSerialization, so inside a captured step
+/* Programmatic dependent launch: every kernel is launched with
+ * cudaLaunchAttributeProgrammaticStreamSerialization, so inside a captured step
  * (common.function, utils/common.py:128 in the reference) the next node's launch overlaps the
  * running one; every kernel orders itself with griddepcontrol.wait. */
-int b200rl_set_pdl(int enabled);
-int b200rl_get_pdl(void);
 
 /* ------------------------------------------------------------------------------------
  * Ring storage — replaces Table (replay_buffers/table.py:32-137) + the variables of
@@ -82,11 +79,6 @@ typedef struct {
   uint32_t* ticket;   /* device scalar uint32 scratch, zero-initialised by the caller */
   b200rl_leaf_t leaves[B200RL_MAX_LEAVES];
 } b200rl_ring_t;
-
-/* Selects the row-copy kernel used by every ring read/write: 0 = 16-byte LDG/STG kernel,
- * 1 = TMA bulk-copy (cp.async.bulk) kernel.  Default: env B200RL_COPY_VARIANT, else 1 (TMA:
- * 5.7 TB/s vs 3.6 TB/s at batch 4096, profiles/r1_gather_sweep.jsonl). */
-int b200rl_set_copy_variant(int variant);
 
 /* _add_batch (tf_uniform_replay_buffer.py:182-209): id = ++last_id; rows[b] = b*L + id % L;
  * scatter every leaf row and the id.  items[i] is a device pointer to [B_env, row_bytes_i]. */
@@ -510,16 +502,6 @@ int b200rl_tc_debug_buffer(long long* dev_buf);
 int b200rl_dense_fwd(const float* X, int64_t ldx, const float* W, const float* bias, float* Y,
                      int64_t M, int64_t K, int64_t N, int act, void* workspace,
                      int64_t ws_bytes, void* stream);
-/* Two dense layers of identical shape (X1 @ W1 + b1 -> Y1, X2 @ W2 + b2 -> Y2; biases both given
- * or both NULL) in one call: b200rl_dense_fwd on each layer in turn, so each layer takes its own
- * route (two launches, plus a split-K reduce each when the shape splits).  DqnAgent evaluates the
- * online network on obs[:, 0] and the target network on obs[:, T-1] this way
- * (agents/dqn/dqn_agent.py:488-520, :575-579 in the reference are the two independent forward
- * passes).  Workspace as b200rl_dense_fwd; the two launches use it one after the other. */
-int b200rl_dense_fwd_pair(const float* X1, const float* X2, int64_t ldx, const float* W1,
-                          const float* W2, const float* bias1, const float* bias2, float* Y1,
-                          float* Y2, int64_t M, int64_t K, int64_t N, int act, void* workspace,
-                          int64_t ws_bytes, void* stream);
 /* Given dY[M,N] (already multiplied by act'), compute dX[M,K] (optional, NULL to skip),
  * dW[K,N] (optional) and db[N] (optional).  accumulate!=0 adds into dW/db instead of
  * overwriting.  x_act: activation code of the layer whose OUTPUT is X (B200RL_ACT_NONE when X is
@@ -527,7 +509,7 @@ int b200rl_dense_fwd_pair(const float* X1, const float* X2, int64_t ldx, const f
  * w.r.t. that layer's pre-activation and no b200rl_act_bwd pass is needed (Keras composes
  * Dense(activation=...) the same way, networks/encoding_network.py:287-300).  In tensor-core
  * mode db is accumulated by the operand producers of the dW GEMM (no separate column-sum
- * launches; B200RL_FUSE_BIAS_GRAD=0 restores them). */
+ * launches). */
 int b200rl_dense_bwd(const float* X, int64_t ldx, const float* W, const float* dY, float* dX,
                      float* dW, float* db, int64_t M, int64_t K, int64_t N, int accumulate,
                      int x_act, void* workspace, int64_t ws_bytes, void* stream);
@@ -546,12 +528,6 @@ typedef struct {
 int b200rl_conv2d_fwd(const void* X, int x_is_u8, float x_scale, const float* Wt,
                       const float* bias, float* Y, const b200rl_conv_t* g, int act,
                       void* workspace, int64_t ws_bytes, void* stream);
-/* Two convolutions of identical geometry in one call: b200rl_conv2d_fwd on each in turn (see
- * b200rl_dense_fwd_pair). */
-int b200rl_conv2d_fwd_pair(const void* X1, const void* X2, int x_is_u8, float x_scale,
-                           const float* Wt1, const float* Wt2, const float* bias1,
-                           const float* bias2, float* Y1, float* Y2, const b200rl_conv_t* c,
-                           int act, void* workspace, int64_t ws_bytes, void* stream);
 /* dX, dW and db may each be NULL (that gradient is skipped), so the parameter gradients and the
  * input gradient of one layer can be issued on different streams.  x_act as in
  * b200rl_dense_bwd: the col2im scatter-add is linear, so act'(X) is applied to every

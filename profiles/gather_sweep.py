@@ -1,5 +1,6 @@
 """Replay gather bandwidth sweep (BASELINE.json configs[4]): rows of 28 244 B, batch 64..4096,
-T=2, 1M-slot ring, LDG kernel (variant 0) vs TMA bulk-copy kernel (variant 1).
+T=2, 1M-slot ring, through the copy kernel the library picks (TMA bulk copy: the 28 224-byte
+observation leaf is 16-byte aligned).
 
 Each point: 20 launches of b200rl_rb_sample captured in one CUDA graph (fresh Philox rows per
 launch, outputs rotate over 4 buffers so no launch rewrites L2-resident lines of the previous
@@ -26,10 +27,8 @@ ROW = 28244
 def main():
   import argparse
   ap = argparse.ArgumentParser()
-  ap.add_argument('--variants', default='0,1')
   ap.add_argument('--batches', default='64,256,1024,4096')
   args = ap.parse_args()
-  variants = [int(v) for v in args.variants.split(',')]
   batches = [int(v) for v in args.batches.split(',')]
   dev = torch.device('cuda:0')
   peak = 6571.6
@@ -64,41 +63,39 @@ def main():
   print(json.dumps(dict(kind='copy_ceiling', gbs=2 * a.numel() * 10 / (e0.elapsed_time(e1) * 1e-3) / 1e9,
                         peak=peak)), flush=True)
   del a, b
-  for variant in variants:
-    _lib.call('b200rl_set_copy_variant', variant)
-    for B in batches:
-      bufs = []
-      for _ in range(nbuf):
-        outs = [torch.empty((B, T) + s.shape, dtype=s.dtype, device=dev) for s in flat]
-        bufs.append((outs, _lib.ptr_array(outs), torch.empty((B, T), dtype=torch.int64, device=dev),
-                     torch.empty(B, dtype=torch.float32, device=dev)))
+  for B in batches:
+    bufs = []
+    for _ in range(nbuf):
+      outs = [torch.empty((B, T) + s.shape, dtype=s.dtype, device=dev) for s in flat]
+      bufs.append((outs, _lib.ptr_array(outs), torch.empty((B, T), dtype=torch.int64, device=dev),
+                   torch.empty(B, dtype=torch.float32, device=dev)))
 
-      def launch(i):
-        outs, ptrs, ids, prob = bufs[i % nbuf]
-        _lib.call('b200rl_rb_sample', ctypes.byref(rb._ring), B, T, None, None, rb._seed,
-                  _lib.ptr(rb._ctrl[0:1]), ptrs, _lib.ptr(ids), None, _lib.ptr(prob),
-                  _lib.ptr(rb._ctrl[1:2]), _lib.stream())
+    def launch(i):
+      outs, ptrs, ids, prob = bufs[i % nbuf]
+      _lib.call('b200rl_rb_sample', ctypes.byref(rb._ring), B, T, None, None, rb._seed,
+                _lib.ptr(rb._ctrl[0:1]), ptrs, _lib.ptr(ids), None, _lib.ptr(prob),
+                _lib.ptr(rb._ctrl[1:2]), _lib.stream())
 
-      for i in range(3):
+    for i in range(3):
+      launch(i)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+      for i in range(nl):
         launch(i)
-      torch.cuda.synchronize()
-      g = torch.cuda.CUDAGraph()
-      with torch.cuda.graph(g):
-        for i in range(nl):
-          launch(i)
+    g.replay()
+    torch.cuda.synchronize()
+    e0.record()
+    for _ in range(reps):
       g.replay()
-      torch.cuda.synchronize()
-      e0.record()
-      for _ in range(reps):
-        g.replay()
-      e1.record()
-      torch.cuda.synchronize()
-      us = e0.elapsed_time(e1) * 1e3 / (nl * reps)
-      nbytes = 2 * B * T * ROW + 8 * B * T
-      gbs = nbytes / (us * 1e-6) / 1e9
-      print(json.dumps(dict(kind='gather', variant='tma' if variant else 'ldg', B=B, T=T, us=us,
-                            gbs=gbs, frac=gbs / peak, bytes=nbytes)), flush=True)
-      del bufs
+    e1.record()
+    torch.cuda.synchronize()
+    us = e0.elapsed_time(e1) * 1e3 / (nl * reps)
+    nbytes = 2 * B * T * ROW + 8 * B * T
+    gbs = nbytes / (us * 1e-6) / 1e9
+    print(json.dumps(dict(kind='gather', B=B, T=T, us=us, gbs=gbs, frac=gbs / peak,
+                          bytes=nbytes)), flush=True)
+    del bufs
 
 
 if __name__ == '__main__':

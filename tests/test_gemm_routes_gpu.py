@@ -206,14 +206,8 @@ CONV_BWD = [
     Conv(*C_F32, (tc(64, 2, ATF, 'BRow'), COL2IM), out_off=1),
     Conv(*C_F32, (tc(64, 2, ATF, 'BRow'), COL2IM), xbs=20 * 20 * 32 + 1),
 ]
-PAIR_DENSE = [
-    Dense(64, 33, 256, (TC_FWD128,)),
-    Dense(33, 1, 20, ('thin_fwd_kernel',)),        # the pair falls back to two single calls
-]
-PAIR_CONV = [Conv(*C_U8, (tc(32, 0, 'AConvU8Raw', 'BRow'), REDUCE), u8=True)]
 
-TABLES = dict(dense_fwd=DENSE_FWD, dense_bwd=DENSE_BWD, conv_fwd=CONV_FWD, conv_bwd=CONV_BWD,
-              dense_pair=PAIR_DENSE, conv_pair=PAIR_CONV)
+TABLES = dict(dense_fwd=DENSE_FWD, dense_bwd=DENSE_BWD, conv_fwd=CONV_FWD, conv_bwd=CONV_BWD)
 
 
 # ---- float64 reference and metric -------------------------------------------------------------
@@ -382,20 +376,12 @@ def _kernel_names(fn):
   return [_normalise(n) for n in names] or None
 
 
-def _names_checkable():
-  """The table assumes the default kernel switches (the GEMM mode is pinned by the fixture)."""
-  return all(os.environ.get(v, '1') == '1' for v in ('B200RL_THIN', 'B200RL_SKINNY',
-                                                     'B200RL_FUSE_BIAS_GRAD'))
-
-
 def check_route(table, row, fn):
   """Runs fn once under the profiler; the set of launched kernels must be exactly row.kernels."""
   names = _kernel_names(fn)
   _CHECKED.add((table, row.id))
   if names is None:
     _PROFILER['empty'] = True
-    return
-  if not _names_checkable():
     return
   _OBSERVED.update(names)
   unexpected = sorted({n for n in names if not any(re.fullmatch(p, n) for p in row.kernels)})
@@ -604,60 +590,6 @@ def test_conv_bwd_route(gemm, row):
   errs.finish()
 
 
-# ---- paired forwards --------------------------------------------------------------------------
-def _dense_pair(row, ws, xs, ws_, bs, act, off):
-  ldx = row.ldx or row.K
-  X = [DevBuf(strided_rows(x, ldx), off) for x in xs]
-  W = [DevBuf(w, off) for w in ws_]
-  B = [DevBuf(b, off) if b is not None else None for b in bs]
-  Y = [DevBuf(nans((row.M, row.N)), row.out_off) for _ in xs]
-  _lib.call('b200rl_dense_fwd_pair', X[0].ptr, X[1].ptr, ldx, W[0].ptr, W[1].ptr, ptr(B[0]),
-            ptr(B[1]), Y[0].ptr, Y[1].ptr, row.M, row.K, row.N, act, *ws(row.ws), _lib.stream())
-  return Y
-
-
-def _conv_pair(row, ws, xs, ws_, bs, act, off):
-  X = [DevBuf(strided_images(x, row.xbs), off) for x in xs]
-  W = [DevBuf(w, off) for w in ws_]
-  B = [DevBuf(b, off) if b is not None else None for b in bs]
-  Y = [DevBuf(nans((row.N * row.oh * row.ow, row.F)), row.out_off) for _ in xs]
-  g = _geom(row)
-  _lib.call('b200rl_conv2d_fwd_pair', X[0].ptr, X[1].ptr, int(row.u8), U8_SCALE, W[0].ptr, W[1].ptr,
-            ptr(B[0]), ptr(B[1]), Y[0].ptr, Y[1].ptr, ctypes.byref(g), act, *ws(), _lib.stream())
-  return Y
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('table,row', [('dense_pair', r) for r in PAIR_DENSE] +
-                         [('conv_pair', r) for r in PAIR_CONV],
-                         ids=[f'dense_{r.id}' for r in PAIR_DENSE] + [f'conv_{r.id}' for r in PAIR_CONV])
-def test_pair_route(gemm, table, row):
-  """Both outputs of a paired forward against their own reference (different weights)."""
-  conv = table == 'conv_pair'
-  errs = Errors(table, row)
-  K = row.k * row.k * row.C if conv else row.K
-  for fam in FAMILIES:
-    rng = rng_for(row.id, fam)
-    if conv:
-      xs = [_conv_input(rng, fam, row) for _ in range(2)]
-      cols = [im2col(_as_f64(x), row.k, row.s) for x in xs]
-    else:
-      xs = cols = [data(rng, fam, (row.M, row.K)) for _ in range(2)]
-    ws_ = [data(rng, fam, (K, row.N if not conv else row.F)) for _ in range(2)]
-    bs = [data(rng, fam, (ws_[0].shape[1],)) for _ in range(2)]
-    zs = [mm(c, w) for c, w in zip(cols, ws_)]
-    run = _conv_pair if conv else _dense_pair
-    if fam == FAMILIES[0]:
-      check_route(table, row, lambda: run(row, gemm, xs, ws_, bs, NONE, 0))
-    for off, bias, act in itertools.product((0, 1), (True, False), ACTS):
-      bb = bs if bias else [None, None]
-      Y = run(row, gemm, xs, ws_, bb, act, off)
-      for i in range(2):
-        errs.add(f'{fam} off={off} bias={bias} act={act}', f'Y{i + 1}', Y[i],
-                 *act_out(zs[i][0], zs[i][1], bb[i], act))
-  errs.finish()
-
-
 # ---- the bound can fail -----------------------------------------------------------------------
 @pytest.mark.gpu
 def test_single_pass_tf32_exceeds_bound(gemm):
@@ -678,11 +610,8 @@ def test_single_pass_tf32_exceeds_bound(gemm):
 
 
 def _run_route_test(gemm, table, row):
-  if table in ('dense_pair', 'conv_pair'):
-    test_pair_route(gemm, table, row)
-  else:
-    dict(dense_fwd=test_dense_fwd_route, dense_bwd=test_dense_bwd_route, conv_fwd=test_conv_fwd_route,
-         conv_bwd=test_conv_bwd_route)[table](gemm, row)
+  dict(dense_fwd=test_dense_fwd_route, dense_bwd=test_dense_bwd_route, conv_fwd=test_conv_fwd_route,
+       conv_bwd=test_conv_bwd_route)[table](gemm, row)
 
 
 @pytest.mark.gpu
@@ -693,8 +622,6 @@ def test_every_listed_kernel_was_observed(gemm):
   The verdict does not depend on what else ran in this process: rows whose route test did not run
   here (a -k selection, or a suite split across processes) run now, and if the profiler saw no
   kernel events earlier, every row runs again under a fresh profiler session."""
-  if not _names_checkable():
-    pytest.skip('kernel names unavailable under non-default kernel switches')
   if _PROFILER['empty']:
     _PROFILER['empty'] = False
     todo = [(t, r) for t, tab in TABLES.items() for r in tab]

@@ -154,32 +154,3 @@ def test_mnih_q_network_forward_backward(cuda):
   wg = orc.backward(wtape, dq)
   for g, w in zip(net._grad_views, wg):
     _close(g, w, rtol=2e-4, tag='mnih_net_grads_b8')   # 4 layers deep: errors of the dX chain compound
-
-
-def test_forward_pair_matches_separate_forwards(cuda):
-  """Network.forward_pair (online + target network, one launch per layer pair) returns what the
-  two separate forward passes return, and its tape back-propagates like forward_train's."""
-  obs_spec = tensor_spec.TensorSpec((44, 44, 4), torch.uint8)
-  act_spec = tensor_spec.BoundedTensorSpec((), torch.int32, 0, 5)
-
-  def make(seed):
-    n = q_network.QNetwork(obs_spec, act_spec, preprocessing_layers=L.CastScale(255.),
-                           conv_layer_params=((16, 8, 4), (32, 4, 2)), fc_layer_params=(64,),
-                           device=cuda).set_seed(seed)
-    n.create_variables()
-    return n
-  online, target = make(1), make(2)
-  assert online.pairs_with(target)
-  g = torch.Generator(device=cuda).manual_seed(0)
-  x = torch.randint(0, 256, (64, 2, 44, 44, 4), dtype=torch.uint8, device=cuda, generator=g)
-  x0, x1 = x[:, 0], x[:, 1]                       # batch-strided views, read in place
-  (q, tape), qt = online.forward_pair(target, x0, x1)
-  q_ref, tape_ref = online.forward_train(x0)
-  qt_ref, _ = target(x1)
-  _close(q, q_ref.cpu().numpy(), rtol=1e-5)
-  _close(qt, qt_ref.cpu().numpy(), rtol=1e-5)
-  assert float((q - qt).abs().max()) > 1e-3      # the two problems really used different weights
-  dq = torch.randn(64, 6, device=cuda, generator=g)
-  g_pair = online.backward(tape, dq).clone()
-  g_ref = online.backward(tape_ref, dq).clone()
-  _close(g_pair, g_ref.cpu().numpy(), rtol=1e-4, tag='paired_vs_separate_grads')   # two atomic orders
