@@ -884,9 +884,9 @@ static int launch_tc_cfg(const AL& a, const BL& b, const GemmArgs& g, const tc::
     configured = true;
   }
   const int64_t tm = (g.M + tc::kBM - 1) / tc::kBM, tn = (g.N + BN - 1) / BN;
-  // one resident CTA per SM: only split when a whole extra set of CTAs fits on the chip.  The
-  // atomic and col2im epilogues add their partials in place; only EPI_STORE needs the workspace.
-  const SplitK sk = plan_split_k(tm * tn, g.K, tc::kBK, kNumSMs, false,
+  // kCtasPerSM resident CTAs per SM: only split when a whole extra set of CTAs fits on the chip.
+  // The atomic and col2im epilogues add their partials in place; only EPI_STORE needs the workspace.
+  const SplitK sk = plan_split_k(tm * tn, g.K, tc::kBK, kNumSMs * L::kCtasPerSM, false,
                                  EPI == tc::EPI_STORE ? g.ws_slices() : 65535);
   B200RL_CHECK_ARG(tm <= 65535, "tc_gemm: M too large for grid.y (%lld tiles)", (long long)tm);
   dim3 grid((unsigned)tn, (unsigned)tm, (unsigned)sk.splits);

@@ -20,6 +20,8 @@
 //   issues wgmma.m64nBNk8 for rows 64w..64w+63 (4 K steps x up to 3 passes per 32-wide K block)
 //   and keeps one group in flight while the next block is split.  Two plane stages: the first
 //   barrier of block i comes after every warpgroup retired the MMAs of block i-2.
+//   Exact A views (raw uint8 pixels) have no A plane: each thread loads its wgmma fragments of A
+//   from the raw ring slot into one of two register sets and only B is split.
 //   The epilogue parks the accumulators in the idle planes / ring and drains them row-per-thread:
 //   bias / activation / act' mask / split-K partials, the fused col2im scatter-add, or red.add.
 #pragma once
@@ -106,6 +108,50 @@ __device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t a, uint
         "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(a), "l"(b), "r"(scale_d));
 }
+// The same MMA with A from registers: a[] is this thread's m64k8 fragment (fp32 bit patterns, see
+// load_frag_*).
+// The registers must not change until a wait_group retires the MMA.
+template <int N>
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b,
+                                              int scale_d);
+template <>
+__device__ __forceinline__ void wgmma_tf32_rs<32>(float (&d)[16], const uint32_t (&a)[4], uint64_t b,
+                                                  int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32_rs<64>(float (&d)[32], const uint32_t (&a)[4], uint64_t b,
+                                                  int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32_rs<128>(float (&d)[64], const uint32_t (&a)[4], uint64_t b,
+                                                   int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d));
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -150,16 +196,30 @@ __device__ __forceinline__ void split_store1(unsigned char* hi_tile, unsigned ch
     asm volatile("st.shared.f32 [%0], %1;" ::"r"(smem_addr(lo_tile) + off), "f"(v - h) : "memory");
 }
 
+// K blocks of raw operand tiles that fit next to `fixed` bytes when `ctas` CTAs share an SM
+constexpr int ring_depth(int fixed, int raw_stage, int ctas) {
+  return (kSmemPerSM / ctas - kSmemPerCta - fixed) / raw_stage;
+}
+// `ctas` CTAs per SM fit when each keeps a ring >= 4 deep and the registers a thread holds across
+// the K loop (accumulators, chain sums, A fragment sets: loop_regs) take at most half of its share
+// of the 64 K register file; the other half goes to addresses, offsets and loop state (tighter
+// bounds spill, see -Xptxas -v).
+constexpr bool ctas_fit(int ctas, int fixed, int raw_stage, int loop_regs) {
+  return ring_depth(fixed, raw_stage, ctas) >= 4 && 2 * loop_regs <= 65536 / (kThreads * ctas);
+}
+
 // A_EXACT: the A view yields values that are exactly representable in TF32 (raw uint8 pixels), so
-// A needs no "lo" plane and the product needs only 2 passes (a*b_lo + a*b_hi).
+// A needs no "lo" part and the product needs only 2 passes (a*b_lo + a*b_hi).  Such A operands go
+// to the MMAs from registers, loaded straight from the raw ring slot, so they have no plane.
 // Shared memory: [kPlaneStages x split planes][kRing x raw operand tiles][bias slice].  The ring is
-// as deep as the opt-in limit allows (at most kMaxRing); a layout whose ring can still be >= 4
-// deep in half an SM runs 2 CTAs per SM (kCtasPerSM, the kernel's launch bound).
+// as deep as the opt-in limit allows (at most kMaxRing) when one CTA runs per SM; a layout that
+// fits 3 or 2 CTAs per SM (ctas_fit) runs that many (kCtasPerSM, the kernel's launch bound), each
+// with the ring of its share.
 template <int BN, int PASSES, bool A_EXACT = false>
 struct SmemLayout {
   static constexpr int kATile = kBM * 128;
   static constexpr int kBTile = BN * 128;
-  static constexpr int kNumA = (PASSES == 3 && !A_EXACT) ? 2 : 1;   // A planes
+  static constexpr int kNumA = A_EXACT ? 0 : PASSES == 3 ? 2 : 1;   // A planes
   static constexpr int kNumB = PASSES == 3 ? 2 : 1;                 // B planes
   static constexpr int kStage = kNumA * kATile + kNumB * kBTile;
   static constexpr int kPlanes = kPlaneStages * kStage;
@@ -168,9 +228,13 @@ struct SmemLayout {
   static constexpr int kRawB = kBK * (BN * 4 + 16);
   static constexpr int kRawStage = kRawA + kRawB;
   static constexpr int kFixed = kPlanes + 1024 /*alignment slack*/ + BN * 4 /*bias*/;
-  static constexpr int kRing2 = (kSmemPerSM / 2 - kSmemPerCta - kFixed) / kRawStage;
-  static constexpr int kCtasPerSM = kRing2 >= 4 ? 2 : 1;
-  static constexpr int kRingFit = kCtasPerSM == 2 ? kRing2 : (kSmemOptIn - kFixed) / kRawStage;
+  // accumulators + chain sums (BN / 2 each) + two A fragment sets of kBK / 8 K steps x 4
+  static constexpr int kLoopRegs = BN + (A_EXACT ? 2 * (kBK / 8) * 4 : 0);
+  static constexpr int kCtasPerSM = ctas_fit(3, kFixed, kRawStage, kLoopRegs)   ? 3
+                                    : ctas_fit(2, kFixed, kRawStage, kLoopRegs) ? 2
+                                                                                : 1;
+  static constexpr int kRingFit = kCtasPerSM > 1 ? ring_depth(kFixed, kRawStage, kCtasPerSM)
+                                                 : (kSmemOptIn - kFixed) / kRawStage;
   static constexpr int kRing = kRingFit < kMaxRing ? kRingFit : kMaxRing;
   static_assert(kRing >= 2, "the operand ring needs two stages");
   static constexpr int kPitch = BN + 4;                             // epilogue staging row (floats)
@@ -330,7 +394,62 @@ struct MnMap {
   __device__ static __forceinline__ int cm(int c) { return (c >> 3) % CPR; }
   __device__ static __forceinline__ int kk(int c) { return (c & 7) | (((c >> 3) / CPR) << 3); }
 };
-template <int ROWS, bool WITH_LO, class V>
+// Register A fragments of raw uint8 tiles.  Fragment of K step ks (wgmma m64k8, tf32): a[0] / a[1]
+// = rows R / R + 8 at column t, a[2] / a[3] = the same rows at column t + 4, with R = 64 wg +
+// 16 (warp % 4) + lane / 4 and t = lane % 4.  Values 0..255 are exact in fp32 and TF32:
+// byte | 0x4B000000 is the float 2^23 + byte.
+__device__ __forceinline__ uint32_t u8_to_f32(uint32_t w, int byte) {
+  return __float_as_uint(__uint_as_float(__byte_perm(w, 0x4B000000u, 0x7540u + (uint32_t)byte)) - 8388608.f);
+}
+// K-contiguous tiles (32-byte rows): four 4-byte loads per block.  That needs the reduction index
+// inside a K block reordered: raw byte p of a row is column kperm(p) of the block's MMAs, so that
+// byte b of word t + 4 h of a row (h < 2) is K step 2 h + b / 2, column t + 4 (b % 2), and every
+// byte of the two words a thread loads per row is one of its fragment values.  The split of B
+// (split_tile_mn<..., true>) stores B in the same order; the permutation keeps its stores at
+// 2-way bank conflicts, and the words a warp loads are 2-way as well.
+__device__ __forceinline__ uint32_t kperm(uint32_t p) {
+  return ((p >> 4) << 4) | (((p >> 1) & 1u) << 3) | ((p & 1u) << 2) | ((p >> 2) & 3u);
+}
+__device__ __forceinline__ void load_frag_k(uint32_t raw, uint32_t (&a)[kBK / 8][4], int wg, int warp,
+                                            int lane) {
+  const uint32_t r = (uint32_t)(wg * 64 + (warp & 3) * 16 + (lane >> 2)), t = (uint32_t)(lane & 3);
+  uint32_t w[2][2];   // [word t / t + 4][row R / R + 8]
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr)
+      asm volatile("ld.shared.u32 %0, [%1];"
+                   : "=r"(w[h][rr]) : "r"(raw + (r + 8u * rr) * 32u + (t + 4u * h) * 4u) : "memory");
+#pragma unroll
+  for (int ks = 0; ks < kBK / 8; ++ks) {
+    const int h = ks >> 1, b = 2 * (ks & 1);
+    a[ks][0] = u8_to_f32(w[h][0], b);
+    a[ks][1] = u8_to_f32(w[h][1], b);
+    a[ks][2] = u8_to_f32(w[h][0], b + 1);
+    a[ks][3] = u8_to_f32(w[h][1], b + 1);
+  }
+}
+// MN-contiguous tiles ([32 k][ROWS + 16] bytes): one byte load per element, natural K order (the
+// 4 t lanes of a load hit k-rows 144 bytes = 4 banks apart, so a load is conflict-free).
+template <int ROWS>
+__device__ __forceinline__ void load_frag_mn(uint32_t raw, uint32_t (&a)[kBK / 8][4], int wg, int warp,
+                                             int lane) {
+  constexpr uint32_t kPitch = ROWS + 16;
+  const uint32_t r = (uint32_t)(wg * 64 + (warp & 3) * 16 + (lane >> 2)), t = (uint32_t)(lane & 3);
+#pragma unroll
+  for (int ks = 0; ks < kBK / 8; ++ks) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const uint32_t k = 8u * ks + t + 4u * (i >> 1), m = r + 8u * (i & 1);
+      uint32_t x;
+      asm volatile("ld.shared.u8 %0, [%1];" : "=r"(x) : "r"(raw + k * kPitch + m) : "memory");
+      a[ks][i] = __float_as_uint(__uint_as_float(x | 0x4B000000u) - 8388608.f);
+    }
+  }
+}
+
+// KPERM: store column k at kperm(k) (B of a K-contiguous register A operand, see load_frag_k).
+template <int ROWS, bool WITH_LO, class V, bool KPERM = false>
 __device__ __forceinline__ void split_tile_mn(const V& v, uint32_t raw, unsigned char* hi,
                                               unsigned char* lo, int tid, bool do_colsum,
                                               float4& colsum) {
@@ -344,7 +463,8 @@ __device__ __forceinline__ void split_tile_mn(const V& v, uint32_t raw, unsigned
     if (do_colsum) {
       colsum.x += x.x; colsum.y += x.y; colsum.z += x.z; colsum.w += x.w;
     }
-    const uint32_t j = k >> 2, e = (k & 3u) * 4u;
+    const uint32_t kc = KPERM ? kperm(k) : k;
+    const uint32_t j = kc >> 2, e = (kc & 3u) * 4u;
     split_store1<WITH_LO>(hi, lo, sw128(r + 0, j) + e, x.x);
     split_store1<WITH_LO>(hi, lo, sw128(r + 1, j) + e, x.y);
     split_store1<WITH_LO>(hi, lo, sw128(r + 2, j) + e, x.z);
@@ -470,57 +590,106 @@ tc_gemm_kernel(const AL a, const BL b, const EpiArgs epi, float* __restrict__ C,
   // the ring's first kRing - 1 blocks are in flight before the loop starts
 #pragma unroll 1
   for (int blk = 0; blk < L::kRing - 1; ++blk) issue(blk);
+  if constexpr (AL::kExact) {
+    // A from registers: each thread loads its fragments of block kbi from the raw ring slot into
+    // set kbi % 2 while block kbi - 1's MMAs (set (kbi - 1) % 2) may still run; the wait_group 1
+    // of block kbi - 1 retired block kbi - 2, the last reader of set kbi % 2.  Blocks go in pairs
+    // so that the set (and the plane stage) is a compile-time index.
+    static_assert(!BL::kKContig, "register A operands pair with an MN-contiguous B view");
+    constexpr bool kPerm = AL::kKContig;
+    uint32_t af[2][kBK / 8][4];
 #pragma unroll 1
-  for (int kbi = 0; kbi < nkb; ++kbi) {
-    // this thread's copies of block kbi have landed; the barrier makes everyone's visible, and it
-    // frees the ring slot of block kbi - 1 (split before the last barrier) and plane stage
-    // kbi % 2 (its MMAs, block kbi - 2, retired in every warpgroup's wait_group 1 below)
-    cp_async_wait<L::kRing - 2>();
-    __syncthreads();
-    issue(kbi + L::kRing - 1);
-    const int s = kbi % kPlaneStages;
-    const uint32_t raw = ring_base + (uint32_t)(kbi % L::kRing) * L::kRawStage;
-    unsigned char* st = smem + s * L::kStage;
-    unsigned char* a_hi = st;
-    unsigned char* a_lo = st + L::kATile;
-    unsigned char* b_hi = st + L::kNumA * L::kATile;
-    unsigned char* b_lo = b_hi + L::kBTile;
-    if constexpr (AL::kKContig) split_tile_k<kBM, kLoA>(a, raw, a_hi, a_lo, tid);
-    else split_tile_mn<kBM, kLoA>(a, raw, a_hi, a_lo, tid, false, bsum);
-    if constexpr (BL::kKContig) split_tile_k<BN, kLo>(b, raw + L::kRawA, b_hi, b_lo, tid);
-    else split_tile_mn<BN, kLo>(b, raw + L::kRawA, b_hi, b_lo, tid, do_colsum, bsum);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic stores -> async proxy
-    __syncthreads();
-    const uint32_t sa = smem_base + (uint32_t)s * L::kStage + (uint32_t)wg * (64u * 128u);
-    const uint32_t sb = smem_base + (uint32_t)s * L::kStage + L::kNumA * L::kATile;
-    const uint32_t a_lo_off = L::kATile, b_lo_off = L::kBTile;
-    const bool fresh = CHAINS && kbi % kChainBlocks == 0;   // first block of a chain
-    if constexpr (CHAINS) {
-      if (fresh && kbi > 0) {
-        // the previous block's MMAs ran during this block's split; usually retired
-        wgmma_wait<0>();
+    for (int kb2 = 0; kb2 < nkb; kb2 += 2) {
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) sum[i] += acc[i];
+      for (int h = 0; h < 2; ++h) {
+        const int kbi = kb2 + h;
+        if (kbi >= nkb) break;
+        cp_async_wait<L::kRing - 2>();
+        __syncthreads();
+        issue(kbi + L::kRing - 1);
+        const uint32_t raw = ring_base + (uint32_t)(kbi % L::kRing) * L::kRawStage;
+        if constexpr (AL::kKContig) load_frag_k(raw, af[h], wg, warp, lane);
+        else load_frag_mn<kBM>(raw, af[h], wg, warp, lane);
+        unsigned char* b_hi = smem + h * L::kStage;
+        split_tile_mn<BN, kLo, BL, kPerm>(b, raw + L::kRawA, b_hi, b_hi + L::kBTile, tid, do_colsum,
+                                          bsum);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        __syncthreads();
+        const uint32_t sb = smem_base + (uint32_t)h * L::kStage;
+        const bool fresh = CHAINS && kbi % kChainBlocks == 0;
+        if constexpr (CHAINS) {
+          if (fresh && kbi > 0) {
+            wgmma_wait<0>();
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) sum[i] += acc[i];
+          }
+        }
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < kBK / 8; ++ks) {
+          const uint32_t ko = (uint32_t)ks * 32u;
+          const int keep = (fresh && ks == 0) ? 0 : 1;
+          if (PASSES == 3) {
+            wgmma_tf32_rs<BN>(acc, af[h][ks], make_desc(sb + L::kBTile + ko), keep);
+            wgmma_tf32_rs<BN>(acc, af[h][ks], make_desc(sb + ko), 1);
+          } else {
+            wgmma_tf32_rs<BN>(acc, af[h][ks], make_desc(sb + ko), keep);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
       }
     }
-    wgmma_fence();
+  } else {
+#pragma unroll 1
+    for (int kbi = 0; kbi < nkb; ++kbi) {
+      // this thread's copies of block kbi have landed; the barrier makes everyone's visible, and it
+      // frees the ring slot of block kbi - 1 (split before the last barrier) and plane stage
+      // kbi % 2 (its MMAs, block kbi - 2, retired in every warpgroup's wait_group 1 below)
+      cp_async_wait<L::kRing - 2>();
+      __syncthreads();
+      issue(kbi + L::kRing - 1);
+      const int s = kbi % kPlaneStages;
+      const uint32_t raw = ring_base + (uint32_t)(kbi % L::kRing) * L::kRawStage;
+      unsigned char* st = smem + s * L::kStage;
+      unsigned char* a_hi = st;
+      unsigned char* a_lo = st + L::kATile;
+      unsigned char* b_hi = st + L::kNumA * L::kATile;
+      unsigned char* b_lo = b_hi + L::kBTile;
+      if constexpr (AL::kKContig) split_tile_k<kBM, kLoA>(a, raw, a_hi, a_lo, tid);
+      else split_tile_mn<kBM, kLoA>(a, raw, a_hi, a_lo, tid, false, bsum);
+      if constexpr (BL::kKContig) split_tile_k<BN, kLo>(b, raw + L::kRawA, b_hi, b_lo, tid);
+      else split_tile_mn<BN, kLo>(b, raw + L::kRawA, b_hi, b_lo, tid, do_colsum, bsum);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic stores -> async proxy
+      __syncthreads();
+      const uint32_t sa = smem_base + (uint32_t)s * L::kStage + (uint32_t)wg * (64u * 128u);
+      const uint32_t sb = smem_base + (uint32_t)s * L::kStage + L::kNumA * L::kATile;
+      const uint32_t a_lo_off = L::kATile, b_lo_off = L::kBTile;
+      const bool fresh = CHAINS && kbi % kChainBlocks == 0;   // first block of a chain
+      if constexpr (CHAINS) {
+        if (fresh && kbi > 0) {
+          // the previous block's MMAs ran during this block's split; usually retired
+          wgmma_wait<0>();
 #pragma unroll
-    for (int ks = 0; ks < kBK / 8; ++ks) {
-      const uint32_t ko = (uint32_t)ks * 32u;   // 8 tf32 = 32 bytes further inside the 128 B row
-      const int keep = (fresh && ks == 0) ? 0 : 1;   // scale-d of the block's first MMA
-      if (PASSES == 3 && AL::kExact) {
-        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + b_lo_off + ko), keep);
-        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko), 1);
-      } else if (PASSES == 3) {
-        wgmma_tf32<BN>(acc, make_desc(sa + a_lo_off + ko), make_desc(sb + ko), keep);
-        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + b_lo_off + ko), 1);
-        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko), 1);
-      } else {
-        wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko), keep);
+          for (int i = 0; i < BN / 2; ++i) sum[i] += acc[i];
+        }
       }
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < kBK / 8; ++ks) {
+        const uint32_t ko = (uint32_t)ks * 32u;   // 8 tf32 = 32 bytes further inside the 128 B row
+        const int keep = (fresh && ks == 0) ? 0 : 1;   // scale-d of the block's first MMA
+        if (PASSES == 3) {
+          wgmma_tf32<BN>(acc, make_desc(sa + a_lo_off + ko), make_desc(sb + ko), keep);
+          wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + b_lo_off + ko), 1);
+          wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko), 1);
+        } else {
+          wgmma_tf32<BN>(acc, make_desc(sa + ko), make_desc(sb + ko), keep);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
     }
-    wgmma_commit();
-    wgmma_wait<1>();
   }
   wgmma_wait<0>();
   if constexpr (CHAINS) {
