@@ -106,6 +106,12 @@ SIGNATURES = {
     'b200rl_sac_actor_loss': [_P, _P, _P, _P, _P, c_i64, c_f32, c_f32, _P, _P, _P, _P, _P, _P],
     'b200rl_sac_alpha_loss': [_P, _P, _P, c_i64, c_f32, c_int, c_f32, c_f32, _P, _P, _P, _P],
     'b200rl_concat2': [_P, c_i64, c_i64, _P, c_i64, c_i64, c_i64, _P, _P],
+    'b200rl_td3_scale_to_spec': [_P, c_i64, c_i64, c_i64, _P, _P, c_f32, c_f32, _P, c_u64, _P, c_int,
+                                 _P, c_i64, _P],
+    'b200rl_td3_critic_loss': [_P, _P, _P, _P, _P, _P, _P, c_i64, c_f32, c_f32, c_int, _P, _P, _P,
+                               _P, _P, _P],
+    'b200rl_td3_actor_loss': [_P, _P, c_i64, _P, _P, _P, _P],
+    'b200rl_td3_actor_bwd': [_P, c_i64, _P, _P, c_i64, c_i64, _P, _P],
     'b200rl_cql_candidates': [_P, c_i64, c_i64, c_i64, c_i64, c_i64, _P, _P, _P, c_u64, _P, _P, _P,
                               _P, _P],
     'b200rl_cql_reward_noise': [_P, c_i64, _P, _P, c_u64, _P, _P, _P],
@@ -132,6 +138,8 @@ SIGNATURES = {
     'b200rl_conv2d_bwd': [_P, c_int, c_f32, _P, _P, _P, _P, _P, ctypes.POINTER(ConvGeom), c_int,
                           c_int, _P, c_i64, _P],
     'b200rl_adam_tf': [_P, _P, _P, _P, c_i64, c_f32, c_f32, c_f32, c_f32, _P, _P, _P],
+    'b200rl_adam_tf_gated': [_P, _P, _P, _P, c_i64, c_f32, c_f32, c_f32, c_f32, _P, _P, _P, c_i64,
+                             _P],
     'b200rl_rmsprop_tf': [_P, _P, _P, _P, _P, c_i64, c_f32, c_f32, c_f32, c_f32, c_int, _P, _P],
     'b200rl_soft_update': [_P, _P, c_i64, c_f32, c_i64, _P, _P],
     'b200rl_clip_by_norm_segments': [_P, _P, c_i64, c_f32, _P],

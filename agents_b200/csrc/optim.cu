@@ -25,13 +25,18 @@ __device__ __forceinline__ void last_block_store(int64_t* ctr, int64_t new_value
   }
 }
 
+// kGated: every block returns before touching anything unless *gate % gate_period == 0, so a
+// skipped update leaves p, m, v and the step counter as they were.
+template <bool kGated>
 __global__ void __launch_bounds__(256) adam_tf_kernel(float* __restrict__ p,
                                                       const float* __restrict__ g,
                                                       float* __restrict__ m,
                                                       float* __restrict__ v, int64_t n, float lr,
                                                       float b1, float b2, float eps,
-                                                      int64_t* step, const float* grad_scale) {
+                                                      int64_t* step, const float* grad_scale,
+                                                      const int64_t* gate, int64_t gate_period) {
   pdl_prologue();
+  if (kGated && gate[0] % gate_period != 0) return;
   __shared__ float s_lr_t;
   const int64_t t = step[0] + 1;
   if (threadIdx.x == 0) {
@@ -211,8 +216,20 @@ int b200rl_adam_tf(float* p, const float* g, float* m, float* v, int64_t n, floa
                    const float* grad_scale_dev, void* stream) {
   B200RL_CHECK_ARG(p && g && m && v && step_dev && n >= 0, "adam_tf: bad argument");
   if (n == 0) return B200RL_OK;
-  B200RL_LAUNCH(adam_tf_kernel, flat_grid(n), 256, 0, (cudaStream_t)stream, p, g, m, v, n, lr, b1, b2, eps, step_dev, grad_scale_dev);
+  B200RL_LAUNCH(adam_tf_kernel<false>, flat_grid(n), 256, 0, (cudaStream_t)stream, p, g, m, v, n, lr, b1, b2, eps, step_dev, grad_scale_dev, (const int64_t*)nullptr, (int64_t)1);
   B200RL_CHECK_LAUNCH("adam_tf");
+  return B200RL_OK;
+}
+
+int b200rl_adam_tf_gated(float* p, const float* g, float* m, float* v, int64_t n, float lr,
+                         float b1, float b2, float eps, int64_t* step_dev,
+                         const float* grad_scale_dev, const int64_t* gate_counter_dev,
+                         int64_t gate_period, void* stream) {
+  B200RL_CHECK_ARG(p && g && m && v && step_dev && n >= 0, "adam_tf_gated: bad argument");
+  B200RL_CHECK_ARG(gate_counter_dev && gate_period >= 1, "adam_tf_gated: bad gate");
+  if (n == 0) return B200RL_OK;
+  B200RL_LAUNCH(adam_tf_kernel<true>, flat_grid(n), 256, 0, (cudaStream_t)stream, p, g, m, v, n, lr, b1, b2, eps, step_dev, grad_scale_dev, gate_counter_dev, gate_period);
+  B200RL_CHECK_LAUNCH("adam_tf_gated");
   return B200RL_OK;
 }
 

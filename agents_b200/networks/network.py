@@ -208,7 +208,8 @@ class Network(object):
     """Forward that records activations; returns (output, tape)."""
     return self._run(observation, keep=True)
 
-  def backward(self, tape, dy, need_input_grad=False, need_param_grads=True, grad_hook=None):
+  def backward(self, tape, dy, need_input_grad=False, need_param_grads=True, grad_hook=None,
+               zero_grads=True):
     """Back-propagates dLoss/d(output) through `tape`, OVERWRITING flat_grads.
 
     grad_hook(lo, hi): called right after the parameter gradients of a layer have been enqueued,
@@ -219,6 +220,8 @@ class Network(object):
 
     need_input_grad: also return dLoss/d(input) (SAC's actor loss differentiates the critics
     w.r.t. their action input); need_param_grads=False skips the weight gradients (dense only).
+    zero_grads=False accumulates into flat_grads as they are (a network whose tape is run in two
+    parts, the CriticNetwork observation branch).
     Returns flat_grads, or (flat_grads, d_input) when need_input_grad."""
     first = next(i for i, (l, _, _) in enumerate(tape) if l.has_params)
     # Inside a captured graph the parameter gradients (dW GEMM + fused bias column sums) of every
@@ -229,8 +232,8 @@ class Network(object):
     # The flat gradient is zeroed ONCE and every layer accumulates into its views (split-K weight
     # gradients and the fused bias sums are red.global.add epilogues): one fill instead of one
     # memset node per layer.
-    zeroed = not need_param_grads
-    if need_param_grads and side is None:
+    zeroed = not (need_param_grads and zero_grads)
+    if not zeroed and side is None:
       self._grads.zero_()
       zeroed = True
 

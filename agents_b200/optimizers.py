@@ -51,11 +51,20 @@ class AdamOptimizer(Optimizer):
   def iterations(self, params):
     return self._get_slots(params)['step'][0]
 
-  def apply_flat(self, params, grads, grad_scale=None):
+  def apply_flat(self, params, grads, grad_scale=None, gate=None):
+    """gate=(counter, period): apply (and count the step) only when the int64 device `counter`
+    is a multiple of `period`, decided on the device so the call can sit in a captured graph."""
     s = self._get_slots(params)
-    _lib.call('b200rl_adam_tf', _lib.ptr(params), _lib.ptr(grads), _lib.ptr(s['m']),
+    if gate is None:
+      _lib.call('b200rl_adam_tf', _lib.ptr(params), _lib.ptr(grads), _lib.ptr(s['m']),
+                _lib.ptr(s['v']), params.numel(), self.learning_rate, self.beta1, self.beta2,
+                self.epsilon, _lib.ptr(s['step']), _lib.ptr(grad_scale), _lib.stream())
+      return
+    counter, period = gate
+    _lib.call('b200rl_adam_tf_gated', _lib.ptr(params), _lib.ptr(grads), _lib.ptr(s['m']),
               _lib.ptr(s['v']), params.numel(), self.learning_rate, self.beta1, self.beta2,
-              self.epsilon, _lib.ptr(s['step']), _lib.ptr(grad_scale), _lib.stream())
+              self.epsilon, _lib.ptr(s['step']), _lib.ptr(grad_scale), _lib.ptr(counter),
+              int(period), _lib.stream())
 
 
 class Adam(AdamOptimizer):

@@ -6,6 +6,8 @@ collect=True  -> a draw from the distribution: Normal(loc, scale) through b200rl
                  Categorical(logits) through b200rl_categorical_sample (`clip` does not apply).
 collect=False -> the greedy policy, the mode of the distribution: loc for a Normal, the first
                  argmax of the logits for a Categorical (b200rl_epsilon_greedy with epsilon 0).
+A deterministic network (ActorNetwork, `deterministic = True`) gives its scale_to_spec action,
+clamped to the action spec when `clip`; `collect` does not apply.
 Draws use a device {call, ticket} counter, so a captured collect step draws fresh values on every
 replay.  Subclasses record extra `policy_info` through `_info` (PPOPolicy).
 """
@@ -85,6 +87,9 @@ class ActorPolicy(tf_policy.TFPolicy):
 
   def _action(self, time_step, policy_state, seed):
     obs = self._normalized(time_step.observation)
+    if getattr(self._actor_net, 'deterministic', False):
+      act = self._actor_net.action(obs, clip=self._clip)
+      return policy_step.PolicyStep(act, policy_state, self._info(obs, act))
     params = self._actor_net.distribution_params(obs)
     if self._actor_net.discrete:
       act = self._categorical_action(params)

@@ -429,6 +429,35 @@ int b200rl_concat2(const float* a, int64_t lda, int64_t da, const float* b, int6
                    int64_t db, int64_t N, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * TD3 (agents/td3/td3_agent.py, agents/ddpg/actor_network.py)
+ * ---------------------------------------------------------------------------------- */
+/* scale_to_spec of the actor's tanh output y [N, A] (row stride ld_y):
+ * out = (amax+amin)/2 + (amax-amin)/2 * y, plus clip(noise_std * z, +-noise_clip) when
+ * noise_std > 0 (z = noise_in [N, A], or N(0,1) by Philox + Box-Muller with rng_call_dev
+ * uint64[2] {call, ticket}), then clamped to [amin, amax] when clamp.  Written at row stride
+ * ld_out, e.g. into the action columns of a critic's joint input; in place (out == y) is allowed. */
+int b200rl_td3_scale_to_spec(const float* y, int64_t ld_y, int64_t N, int64_t A,
+                             const float* amin, const float* amax, float noise_std,
+                             float noise_clip, const float* noise_in, uint64_t seed,
+                             uint64_t* rng_call_dev, int clamp, float* out, int64_t ld_out,
+                             void* stream);
+/* Twin-critic loss: y = reward_scale*r + gamma*d*min(tq1, tq2); loss = mean_b(w_b*(l(y,q1) +
+ * l(y,q2))) with l = B200RL_LOSS_HUBER (delta 1) or B200RL_LOSS_SQUARED; dq1, dq2 = dloss/dq.
+ * One block, fixed-order reduction.  weights, td_targets and nan_flag may be NULL. */
+int b200rl_td3_critic_loss(const float* q1, const float* q2, const float* tq1, const float* tq2,
+                           const float* reward, const float* discount, const float* weights,
+                           int64_t B, float gamma, float reward_scale, int loss_kind,
+                           float* loss, float* dq1, float* dq2, float* td_targets,
+                           int32_t* nan_flag, void* stream);
+/* Actor loss sum_b(w_b * -q_b) / B and dq = -w / B. */
+int b200rl_td3_actor_loss(const float* q, const float* weights, int64_t B, float* loss,
+                          float* dq, int32_t* nan_flag, void* stream);
+/* dy [N, A] = (amax-amin)/2 * da, da read at row stride ld_da (the action columns of a critic's
+ * input gradient): the gradient w.r.t. the actor's tanh output. */
+int b200rl_td3_actor_bwd(const float* da, int64_t ld_da, const float* amin, const float* amax,
+                         int64_t N, int64_t A, float* dy, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * CQL-SAC (csrc/cql.cu).  Replaces agents/cql/cql_sac_agent.py (_cql_loss :534-679, actor_loss
  * :681-750, _get_cql_alpha :752-765, reward noise :832-839, the Lagrange step of _train
  * :336-348).  The critic joint input x is [B + 2BN, D+A]: rows [0, B) (s, a_data), [B, B+BN) the
@@ -548,6 +577,13 @@ int b200rl_conv2d_bwd(const void* X, int x_is_u8, float x_scale, const float* Wt
 int b200rl_adam_tf(float* p, const float* g, float* m, float* v, int64_t n, float lr,
                    float b1, float b2, float eps, int64_t* step_dev,
                    const float* grad_scale_dev, void* stream);
+/* b200rl_adam_tf gated on the device: the whole update, including the step_dev increment, runs
+ * only when *gate_counter_dev % gate_period == 0 (TD3's delayed actor update inside a captured
+ * train step; gate_counter_dev is the int64 train-step counter). */
+int b200rl_adam_tf_gated(float* p, const float* g, float* m, float* v, int64_t n, float lr,
+                         float b1, float b2, float eps, int64_t* step_dev,
+                         const float* grad_scale_dev, const int64_t* gate_counter_dev,
+                         int64_t gate_period, void* stream);
 /* TF RMSProp (tf.compat.v1.train.RMSPropOptimizer; Mnih'15 config
  * examples/dqn/mnih15/dqn_train_eval_atari.py:176-182): centered optional. */
 int b200rl_rmsprop_tf(float* p, const float* g, float* ms, float* mg, float* mom, int64_t n,
