@@ -29,10 +29,18 @@ def _agent_state_tensors(agent):
   out = {}
   for name in ('_q_network', '_target_q_network', '_actor_net', '_value_net', '_actor_network',
                '_value_network', '_critic_network_1', '_critic_network_2', '_target_critic_network_1',
-               '_target_critic_network_2', '_target_actor_network'):
+               '_target_critic_network_2', '_target_actor_network', '_critic_network',
+               '_target_critic_network'):
     net = getattr(agent, name, None)
     if net is not None and hasattr(net, 'flat_params'):
       out[name] = net.flat_params
+  # OUNoisePolicy's process value and Philox counter (agent-tracked variables in the reference),
+  # so a restored run draws the exploration noise it would have drawn
+  collect = getattr(agent, '_collect_policy', None)
+  for name in ('_ou_state', '_ou_rng'):
+    t = getattr(collect, name, None)
+    if isinstance(t, torch.Tensor):
+      out['_collect_policy/' + name] = t
   # SAC temperature; CQL-SAC's weight (a device scalar, or log_cql_alpha with Lagrange); TD3's
   # target-smoothing Philox counter (a restored run draws the noise it would have drawn)
   for name in ('_log_alpha', '_cql_alpha', '_log_cql_alpha', '_target_noise_rng'):

@@ -458,6 +458,35 @@ int b200rl_td3_actor_bwd(const float* da, int64_t ld_da, const float* amin, cons
                          int64_t N, int64_t A, float* dy, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * DDPG (agents/ddpg/ddpg_agent.py, policies/ou_noise_policy.py, utils/common.py OUProcess).
+ * The target action a' = scale_to_spec(target_actor(s')) comes from b200rl_td3_scale_to_spec.
+ * ---------------------------------------------------------------------------------- */
+/* Single-critic loss: y = reward_scale*r + gamma*d*tq; loss = mean_b(w_b*l(y, q_b)) with
+ * l = B200RL_LOSS_HUBER (delta 1) or B200RL_LOSS_SQUARED; dq = w_b/B * dl/dq.  One block,
+ * fixed-order reduction.  weights, td_targets and nan_flag may be NULL. */
+int b200rl_ddpg_critic_loss(const float* q, const float* tq, const float* reward,
+                            const float* discount, const float* weights, int64_t B, float gamma,
+                            float reward_scale, int loss_kind, float* loss, float* dq,
+                            float* td_targets, int32_t* nan_flag, void* stream);
+/* Actor loss from dQ/da [B, A] read at row stride ld_dqda (the action columns of a critic's input
+ * gradient of sum(Q)): c = clip(dqda, +-dqda_clipping) when clip (0 zeroes c), else dqda;
+ * loss = sum_b w_b sum_k c_bk^2 / (B*A); dy [B, A] = (amax-amin)/2 * (-2 w_b c_bk / (B*A)), the
+ * gradient w.r.t. the actor's tanh output (no gradient through c).  One block, fixed order. */
+int b200rl_ddpg_actor_loss(const float* dqda, int64_t ld_dqda, const float* weights, int64_t B,
+                           int64_t A, int clip, float dqda_clipping, const float* amin,
+                           const float* amax, float* loss, float* dy, int32_t* nan_flag,
+                           void* stream);
+/* One Ornstein-Uhlenbeck step: state [A] <- (1-damping)*state + stddev*z, z = noise_in [A] or
+ * N(0,1) by Philox + Box-Muller on element k of rng_call_dev uint64[2] {call, ticket} (the call
+ * advances only when the device draws; the ticket slot is used either way); then
+ * out[n, k] = loc[n, k] + state[k] for every row, clamped to [amin, amax] when they are given.
+ * The state is advanced exactly once per call, whatever the grid. */
+int b200rl_ou_noise(const float* loc, int64_t ld_loc, int64_t N, int64_t A, float* state,
+                    float damping, float stddev, const float* noise_in, uint64_t seed,
+                    uint64_t* rng_call_dev, const float* amin, const float* amax, float* out,
+                    int64_t ld_out, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * CQL-SAC (csrc/cql.cu).  Replaces agents/cql/cql_sac_agent.py (_cql_loss :534-679, actor_loss
  * :681-750, _get_cql_alpha :752-765, reward noise :832-839, the Lagrange step of _train
  * :336-348).  The critic joint input x is [B + 2BN, D+A]: rows [0, B) (s, a_data), [B, B+BN) the
