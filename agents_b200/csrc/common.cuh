@@ -117,6 +117,29 @@ __host__ __device__ __forceinline__ float uniform_f32(uint32_t a) {
   return (float)(a >> 8) * (1.0f / 16777216.0f);
 }
 
+// N(0, 1) by Box-Muller on one Philox draw (u1 in (0, 1] from x, the angle from y).
+__device__ __forceinline__ float philox_normal(uint64_t elem, uint64_t call, uint64_t seed) {
+  const Philox4 r = philox4x32_10(elem, call, seed);
+  const float u1 = ((float)(r.x >> 8) + 1.0f) * (1.0f / 16777216.0f);
+  return sqrtf(-2.f * logf(u1)) * cospif(2.f * uniform_f32(r.y));
+}
+
+// The last block to finish advances the Philox call counter {call, ticket} (as sac_sample), so a
+// captured graph draws fresh values on every replay.  Every thread of the grid must reach it, and
+// every block must have read rng_call[0] before.
+__device__ __forceinline__ void next_rng_call(uint64_t* rng_call) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    unsigned int tk = atomicAdd((uint32_t*)(rng_call + 1), 1u);
+    if (tk == gridDim.x - 1) {
+      *(uint32_t*)(rng_call + 1) = 0u;
+      rng_call[0] = rng_call[0] + 1;
+      __threadfence();
+    }
+  }
+}
+
 // ---- 16-byte streaming copies -------------------------------------------------------------
 __device__ __forceinline__ int4 ld_stream16(const void* p) {
   int4 r;

@@ -20,21 +20,6 @@ namespace b200rl {
 
 constexpr int kCqlRedBlocks = 256;
 
-// The last block to finish advances the Philox call counter {call, ticket} (as sac_sample), so a
-// captured graph draws fresh values on every replay.
-__device__ __forceinline__ void next_rng_call(uint64_t* rng_call) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    unsigned int tk = atomicAdd((uint32_t*)(rng_call + 1), 1u);
-    if (tk == gridDim.x - 1) {
-      *(uint32_t*)(rng_call + 1) = 0u;
-      rng_call[0] = rng_call[0] + 1;
-      __threadfence();
-    }
-  }
-}
-
 // Tiles the observation into every candidate row, fills the uniform candidates' actions
 // (tf.random.uniform(minval, maxval) = minval + u * (maxval - minval), u in [0, 1)) and tiles the
 // actor head [B, 2A] -> [BN, 2A] for b200rl_sac_sample.  The policy candidates' action columns are

@@ -126,14 +126,7 @@ class CriticNetwork(network.Network):
     action_column + A) of x, so a caller may rewrite it there before `forward_stack`."""
     if not self._n_obs_layers:
       return self.joint_input(observation, action), None
-    self._require_built()
-    obs_tape = []
-    h = observation.float()
-    for l in self._layers[1:1 + self._n_obs_layers]:
-      y = l.forward(h)
-      if keep:
-        obs_tape.append((l, h, y))
-      h = y
+    h, obs_tape = self.observation_features(observation, keep)
     action = action.float()
     if action.stride(1) != 1:
       action = action.contiguous()
@@ -142,6 +135,19 @@ class CriticNetwork(network.Network):
     _lib.call('b200rl_concat2', _lib.ptr(h), hd, hd, _lib.dptr(action), action.stride(0),
               self._act_dim, n, _lib.ptr(x), _lib.stream())
     return x, obs_tape
+
+  def observation_features(self, observation, keep=False):
+    """(h_obs [N, H], obs_tape) of the observation branch, the part of the joint-stack input that
+    does not depend on the action.  Requires an observation branch."""
+    self._require_built()
+    obs_tape = []
+    h = observation.float()
+    for l in self._layers[1:1 + self._n_obs_layers]:
+      y = l.forward(h)
+      if keep:
+        obs_tape.append((l, h, y))
+      h = y
+    return h, obs_tape
 
   def forward_stack(self, x, obs_tape=None, keep=False):
     """(q [N, 1], tape for `backward`) from the joint-stack input `stack_input` returned."""

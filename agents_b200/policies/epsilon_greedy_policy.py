@@ -4,13 +4,19 @@ Reference: policies/epsilon_greedy_policy.py:120-145 (`u ~ U[0, 1)` per batch ro
 branch is `RandomTFPolicy` over the same action mask).  Device work: one b200rl_epsilon_greedy
 launch (greedy_policy._Selecting).  `epsilon` may be a float or a callable evaluated on the host at
 every call (:93-99).
+
+For a bounded float action spec (QtOptAgent's collect policy over CEMPolicy) the wrapped policy's
+action is taken and, per row with probability epsilon, replaced by a uniform draw in
+[minimum, maximum) (one b200rl_epsilon_uniform launch, greedy_policy._FloatUniform).
 """
 import warnings
 
 import torch
 
+from agents_b200.policies.greedy_policy import _FloatUniform
 from agents_b200.policies.greedy_policy import _Selecting
 from agents_b200.trajectories import policy_step
+from agents_b200.utils import nest
 
 
 class EpsilonGreedyPolicy(_Selecting):
@@ -21,6 +27,13 @@ class EpsilonGreedyPolicy(_Selecting):
     self._wrapped_policy = policy
     self._epsilon = epsilon
     self._warned_capture = False
+    self._float = None
+    spec = nest.flatten(policy.action_spec)[0]
+    if spec.dtype.is_floating_point:
+      net = getattr(policy, 'q_network', None)
+      self._float = _FloatUniform(spec, self._seed,
+                                  net.device if net is not None else torch.device('cuda'))
+      self._uniform_rng = self._float.rng
 
   @property
   def wrapped_policy(self):
@@ -43,6 +56,10 @@ class EpsilonGreedyPolicy(_Selecting):
     return self._epsilon()
 
   def _action(self, time_step, policy_state, seed):
+    if self._float is not None:
+      step = self._wrapped_policy.action(time_step, policy_state, seed)
+      act = self._float.apply(step.action.float().clone(), self._get_epsilon())
+      return policy_step.PolicyStep(act, step.state, step.info)
     q, mask = self._wrapped_policy.q_values(time_step)
     act = self._select(q, mask, self._get_epsilon(), self._wrapped_policy._action_dtype)
     return policy_step.PolicyStep(act, policy_state, ())

@@ -6,6 +6,7 @@ the ONE launch (b200rl_epsilon_greedy, csrc/env.cu) behind GreedyPolicy (epsilon
 random), EpsilonGreedyPolicy (epsilon_greedy_policy.py) and RandomTFPolicy (epsilon = 2: always
 random, random_tf_policy.py): Philox draw, masked argmax and masked uniform choice per batch row.
 """
+import numpy as np
 import torch
 
 from agents_b200 import _lib
@@ -34,6 +35,34 @@ class _Selecting(tf_policy.TFPolicy):
               float(eps), self._seed, _lib.ptr(self._rng), None, None, _lib.ptr(out),
               _lib.stream())
     return out if dtype == torch.int32 else out.to(dtype)
+
+
+class _FloatUniform(object):
+  """The float-spec branch shared by EpsilonGreedyPolicy and RandomTFPolicy: one
+  b200rl_epsilon_uniform launch replaces a row, with probability epsilon, by a uniform draw in
+  [minimum, maximum) of a bounded float spec of rank 0 or 1 (tensor_spec.sample_spec_nest).  The
+  Philox counter is a device tensor allocated here, so a captured collect step draws fresh values
+  on every replay."""
+
+  def __init__(self, spec, seed, device):
+    a = int(np.prod(spec.shape)) if len(spec.shape) else 1
+    if len(spec.shape) > 1:
+      raise NotImplementedError('Float actions of rank > 1 are not supported.')
+    self.num_actions = a
+    self.amin = torch.as_tensor(np.broadcast_to(np.asarray(spec.minimum, np.float32), (a,)).copy(),
+                                device=device)
+    self.amax = torch.as_tensor(np.broadcast_to(np.asarray(spec.maximum, np.float32), (a,)).copy(),
+                                device=device)
+    self.seed = seed
+    self.rng = torch.zeros(2, dtype=torch.int64, device=device)
+
+  def apply(self, action, eps):
+    """Overwrites rows of `action` ([N, A], or [N] for a scalar spec) in place."""
+    n = action.shape[0]
+    _lib.call('b200rl_epsilon_uniform', _lib.ptr(action), self.num_actions, n, self.num_actions,
+              float(eps), _lib.ptr(self.amin), _lib.ptr(self.amax), self.seed,
+              _lib.ptr(self.rng), _lib.stream())
+    return action
 
 
 class GreedyPolicy(_Selecting):

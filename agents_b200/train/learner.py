@@ -30,7 +30,8 @@ def _agent_state_tensors(agent):
   for name in ('_q_network', '_target_q_network', '_actor_net', '_value_net', '_actor_network',
                '_value_network', '_critic_network_1', '_critic_network_2', '_target_critic_network_1',
                '_target_critic_network_2', '_target_actor_network', '_critic_network',
-               '_target_critic_network'):
+               '_target_critic_network', '_target_q_network_delayed',
+               '_target_q_network_delayed_2'):
     net = getattr(agent, name, None)
     if net is not None and hasattr(net, 'flat_params'):
       out[name] = net.flat_params
@@ -41,6 +42,14 @@ def _agent_state_tensors(agent):
     t = getattr(collect, name, None)
     if isinstance(t, torch.Tensor):
       out['_collect_policy/' + name] = t
+  # QT-Opt: the Philox counters of the float epsilon-greedy draw and of CEMPolicy's search (the
+  # train step searches with the same policy), so a restored run draws what it would have drawn
+  t = getattr(collect, '_uniform_rng', None)
+  if isinstance(t, torch.Tensor):
+    out['_collect_policy/_uniform_rng'] = t
+  t = getattr(getattr(agent, '_policy', None), '_cem_rng', None)
+  if isinstance(t, torch.Tensor):
+    out['_policy/_cem_rng'] = t
   # SAC temperature; CQL-SAC's weight (a device scalar, or log_cql_alpha with Lagrange); TD3's
   # target-smoothing Philox counter (a restored run draws the noise it would have drawn)
   for name in ('_log_alpha', '_cql_alpha', '_log_cql_alpha', '_target_noise_rng'):
@@ -60,6 +69,10 @@ def _agent_state_tensors(agent):
   upd = getattr(agent, '_update_target', None)       # Periodically counter (a tf.Variable there)
   if isinstance(getattr(upd, '_counter', None), torch.Tensor):
     out['_update_target/counter'] = upd._counter
+  for name in ('_target_updater_delayed', '_target_updater_delayed_2'):   # QT-Opt's delayed chain
+    upd = getattr(agent, name, None)
+    if isinstance(getattr(upd, '_counter', None), torch.Tensor):
+      out[name + '/counter'] = upd._counter
   # optimiser slots are created lazily on the first apply; materialise them for the parameter
   # buffers each agent steps, so that a freshly built agent can be restored into
   pairs = (('_optimizer', '_flat_params'), ('_critic_optimizer', '_critic_params'),

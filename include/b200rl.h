@@ -487,6 +487,54 @@ int b200rl_ou_noise(const float* loc, int64_t ld_loc, int64_t N, int64_t A, floa
                     int64_t ld_out, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * QT-Opt (csrc/qtopt.cu): policies/qtopt_cem_policy.py, the continuous GaussianActionsSampler,
+ * agents/qtopt/qtopt_agent.py, and the float-spec branch of EpsilonGreedyPolicy / RandomTFPolicy.
+ * A CEM search of N samples per state writes its samples into the action columns of a critic's
+ * joint-stack input x [B*N, ld_x]; sample n of state b is row b*N + n (tile_batch order) and
+ * draw (row, k) is z_in[row*A + k] or N(0,1) by Philox + Box-Muller on element row*A + k of the
+ * call rng_call_dev[0] (uint64[2] {call, ticket}; the call advances once per launch that draws
+ * from the device).
+ * ---------------------------------------------------------------------------------- */
+/* First iteration of a search: x[r, c] = src[r/N, c] for c < C (the observation, or h_obs with
+ * an observation branch: the tiling is done once per search), and x[r, C + k] =
+ * clip(mean[b, k] + sqrt(max(var[b, k], minimal_var)) * z, amin[k], amax[k]) for k < A.
+ * ld_mean = ld_var = 0 broadcasts one [A] distribution to every state.  src may be NULL when
+ * C = 0. */
+int b200rl_cem_sample(const float* src, int64_t ld_src, int64_t B, int64_t N, int64_t C,
+                      int64_t A, const float* mean, int64_t ld_mean, const float* var,
+                      int64_t ld_var, float minimal_var, const float* amin, const float* amax,
+                      const float* z_in, uint64_t seed, uint64_t* rng_call_dev, float* x,
+                      int64_t ld_x, void* stream);
+/* End of one iteration, one warp per state: selects the top M of the N scores [B*N] (higher
+ * first, the lower index on a tie, as tf.nn.top_k), refits mean/var [B, A] over the elites'
+ * actions (x columns [col, col+A)) in rank order with tf.nn.moments semantics (mean, then the
+ * mean of squared deviations, both / M).  Unless `last`, draws the next N samples per state into
+ * the same columns (as b200rl_cem_sample); when `last`, writes best_action [B, A] (elite 0's
+ * action) and best_score [B] instead (either may be NULL).  elite_idx [B, M] (optional) replaces
+ * the selection; scores may then be NULL.  1 <= M <= N, M + 2A <= 3072. */
+int b200rl_cem_refit(const float* scores, const int32_t* elite_idx, float* x, int64_t ld_x,
+                     int64_t col, int64_t B, int64_t N, int64_t M, int64_t A, float minimal_var,
+                     const float* amin, const float* amax, int last, const float* z_in,
+                     uint64_t seed, uint64_t* rng_call_dev, float* mean, float* var,
+                     float* best_action, float* best_score, void* stream);
+/* TD loss: next_q = min(tq1, tq2) (tq1 when tq2 is NULL); y = reward_scale*r + gamma*d*next_q;
+ * m_b = (step_type[b*step_stride] != LAST); td_error = m (y - q); td_loss = m l(y, q) with
+ * l = B200RL_LOSS_HUBER (delta 1) or B200RL_LOSS_SQUARED; loss = sum_b w_b td_loss_b / B;
+ * dq = m w_b / B dl/dq.  One block, fixed-order reduction.  weights and nan_flag may be NULL. */
+int b200rl_qtopt_td_loss(const float* q, const float* tq1, const float* tq2, const float* reward,
+                         const float* discount, const int32_t* step_type, int64_t step_stride,
+                         const float* weights, int64_t B, float gamma, float reward_scale,
+                         int loss_kind, float* loss, float* td_loss, float* td_error, float* dq,
+                         int32_t* nan_flag, void* stream);
+/* In place over action [N, A] (row stride ld): row n is replaced where
+ * u_n = uniform_f32(philox(n, call, seed).x) < epsilon by amin + u * (amax - amin) per column
+ * (u from element n*A + k under a second key).  epsilon >= 1 replaces every row (RandomTFPolicy).
+ * The call counter advances on every launch. */
+int b200rl_epsilon_uniform(float* action, int64_t ld, int64_t N, int64_t A, float epsilon,
+                           const float* amin, const float* amax, uint64_t seed,
+                           uint64_t* rng_call_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * CQL-SAC (csrc/cql.cu).  Replaces agents/cql/cql_sac_agent.py (_cql_loss :534-679, actor_loss
  * :681-750, _get_cql_alpha :752-765, reward noise :832-839, the Lagrange step of _train
  * :336-348).  The critic joint input x is [B + 2BN, D+A]: rows [0, B) (s, a_data), [B, B+BN) the
