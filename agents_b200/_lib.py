@@ -123,6 +123,10 @@ SIGNATURES = {
     'b200rl_qtopt_td_loss': [_P, _P, _P, _P, _P, _P, c_i64, _P, c_i64, c_f32, c_f32, c_int, _P, _P,
                              _P, _P, _P, _P],
     'b200rl_epsilon_uniform': [_P, c_i64, c_i64, c_i64, c_f32, _P, _P, c_u64, _P, _P],
+    'b200rl_bc_discrete_loss': [_P, c_i64, _P, c_i64, ctypes.c_int32, _P, c_i64, c_i64, c_i64, _P,
+                                _P, _P, c_i64, _P, _P, c_i64, _P],
+    'b200rl_bc_continuous_loss': [_P, _P, c_i64, _P, c_i64, _P, _P, _P, c_u64, _P, c_int, _P,
+                                  c_i64, c_i64, c_i64, _P, _P, _P, _P, c_i64, _P, _P, c_i64, _P],
     'b200rl_cql_candidates': [_P, c_i64, c_i64, c_i64, c_i64, c_i64, _P, _P, _P, c_u64, _P, _P, _P,
                               _P, _P],
     'b200rl_cql_reward_noise': [_P, c_i64, _P, _P, c_u64, _P, _P, _P],

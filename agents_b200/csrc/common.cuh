@@ -184,6 +184,17 @@ __device__ __forceinline__ float grp_sum(float v) {
   return v;
 }
 
+// Lanes per row of width W: one thread for narrow rows, 8 or 32 lanes once a row spans more than
+// 8 / 64 columns (coalesced row reads, shuffle reductions).
+static inline int lane_group(int64_t width) { return width <= 8 ? 1 : (width <= 64 ? 8 : 32); }
+
+// 256-thread blocks for N rows of G lanes each, at most `cap` (the partials one final block
+// reduces); the group kernels stride over the rest.
+static inline unsigned group_blocks(int64_t N, int G, int64_t cap) {
+  const int64_t nb = (N * G + 255) / 256;
+  return (unsigned)(nb > cap ? cap : nb);
+}
+
 // Row iteration shared by the group kernels: n is this group's row, n0 the row of the warp's first
 // group (warp-uniform loop bound).
 #define B200RL_GROUP_ROWS(G, N)                                                              \

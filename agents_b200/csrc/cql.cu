@@ -263,7 +263,6 @@ __global__ void cql_bc_actor_bwd_kernel(const float* __restrict__ head,
 using namespace b200rl;
 
 static unsigned cql_blocks(int64_t n) { return (unsigned)((n + 255) / 256); }
-static int cql_group(int64_t width) { return width <= 8 ? 1 : (width <= 64 ? 8 : 32); }
 
 extern "C" {
 
@@ -311,12 +310,11 @@ int b200rl_cql_loss(const float* q1, const float* q2, const float* logp, int64_t
   a.cql_alpha = cql_alpha_dev; a.log_cql_alpha = log_cql_alpha_dev;
   a.clip_lo = clip_lo; a.clip_hi = clip_hi; a.bc_debug = bc_debug;
   a.dq1 = dq1; a.dq2 = dq2; a.partial = (float*)workspace;
-  const int G = cql_group(2 * N);
-  int64_t nb = (B * G + 255) / 256;
-  if (nb > kCqlRedBlocks) nb = kCqlRedBlocks;
-  if (G == 1) B200RL_LAUNCH(cql_loss_rows_kernel<1>, (unsigned)nb, 256, 0, st, a);
-  else if (G == 8) B200RL_LAUNCH(cql_loss_rows_kernel<8>, (unsigned)nb, 256, 0, st, a);
-  else B200RL_LAUNCH(cql_loss_rows_kernel<32>, (unsigned)nb, 256, 0, st, a);
+  const int G = lane_group(2 * N);
+  const unsigned nb = group_blocks(B, G, kCqlRedBlocks);
+  if (G == 1) B200RL_LAUNCH(cql_loss_rows_kernel<1>, nb, 256, 0, st, a);
+  else if (G == 8) B200RL_LAUNCH(cql_loss_rows_kernel<8>, nb, 256, 0, st, a);
+  else B200RL_LAUNCH(cql_loss_rows_kernel<32>, nb, 256, 0, st, a);
   B200RL_CHECK_LAUNCH("cql_loss_rows");
   B200RL_LAUNCH(cql_loss_final_kernel, 1, 256, 0, st, (const float*)workspace, (int)nb, B, cql_alpha_dev, log_cql_alpha_dev, clip_lo, clip_hi, cql_tau, bc_debug, critic_loss, out, dlog_cql_alpha, nan_flag);
   B200RL_CHECK_LAUNCH("cql_loss_final");

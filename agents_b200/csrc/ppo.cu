@@ -405,7 +405,7 @@ __global__ void ppo_kl_beta_update_kernel(const float* __restrict__ mean_kl,
 
 // ---- Categorical policy (discrete actions): CategoricalProjectionNetwork logits [N, A] --------
 // A row of logits is handled by a group of G lanes (B200RL_GROUP_ROWS, common.cuh); G follows
-// from A (cat_group): one thread per row for narrow rows, 8 or 32 lanes with shuffle reductions
+// from A (lane_group): one thread per row for narrow rows, 8 or 32 lanes with shuffle reductions
 // for wide ones, so a row is read with coalesced loads.  row_softmax_stats / clamp_action live in
 // common.cuh (shared with reinforce.cu).
 
@@ -706,18 +706,9 @@ int b200rl_normal_sample(const float* loc, const float* scale, int64_t ld, int64
 
 }  // extern "C"
 
-// Lanes per logits row: one thread for narrow rows, 8 or 32 lanes once a row spans more than
-// 8 / 64 columns (coalesced row reads, shuffle reductions).
-static int cat_group(int64_t A) { return A <= 8 ? 1 : (A <= 64 ? 8 : 32); }
-
 // The categorical kernels fill the GPU up to the 512 partials one 512-thread final kernel reduces
 // (about 4 CTAs of 256 per SM; the continuous kernels keep kRedBlocks).
 constexpr int kCatRedBlocks = 512;
-
-static unsigned cat_blocks(int64_t N, int G, int cap) {
-  int64_t nb = (N * G + 255) / 256;
-  return (unsigned)(nb > cap ? cap : nb);
-}
 
 extern "C" {
 
@@ -747,8 +738,8 @@ int b200rl_ppo_loss_categorical(const float* logits, int64_t ld, const int32_t* 
     a.old_logits = kl->old_logits; a.ld_old = kl->ld_old;
     a.kl_terms = kl->terms; a.kl_grad_scale = kl->grad_scale;
   }
-  const int G = cat_group(A);
-  const unsigned nb = cat_blocks(N, G, kCatRedBlocks);
+  const int G = lane_group(A);
+  const unsigned nb = group_blocks(N, G, kCatRedBlocks);
   if (G == 1) B200RL_LAUNCH(ppo_loss_cat_kernel<1>, nb, 256, 0, st, a);
   else if (G == 8) B200RL_LAUNCH(ppo_loss_cat_kernel<8>, nb, 256, 0, st, a);
   else B200RL_LAUNCH(ppo_loss_cat_kernel<32>, nb, 256, 0, st, a);
@@ -764,8 +755,8 @@ int b200rl_categorical_logp(const float* logits, int64_t ld, const int32_t* acti
                    "categorical_logp: bad argument");
   if (N == 0) return B200RL_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const int G = cat_group(A);
-  const unsigned nb = cat_blocks(N, G, 1 << 30);
+  const int G = lane_group(A);
+  const unsigned nb = group_blocks(N, G, 1 << 30);
   if (G == 1) B200RL_LAUNCH(categorical_logp_kernel<1>, nb, 256, 0, st, logits, ld, action, N, A, out, nan_flag);
   else if (G == 8) B200RL_LAUNCH(categorical_logp_kernel<8>, nb, 256, 0, st, logits, ld, action, N, A, out, nan_flag);
   else B200RL_LAUNCH(categorical_logp_kernel<32>, nb, 256, 0, st, logits, ld, action, N, A, out, nan_flag);
@@ -782,8 +773,8 @@ int b200rl_ppo_kl_categorical(const float* logits, int64_t ld, const float* old_
   B200RL_CHECK_ARG(workspace && ws_bytes >= (int64_t)(kCatRedBlocks * sizeof(float)),
                    "ppo_kl_categorical: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
-  const int G = cat_group(A);
-  const unsigned nb = cat_blocks(N, G, kCatRedBlocks);
+  const int G = lane_group(A);
+  const unsigned nb = group_blocks(N, G, kCatRedBlocks);
   float* part = (float*)workspace;
   if (G == 1) B200RL_LAUNCH(ppo_kl_cat_partial_kernel<1>, nb, 256, 0, st, logits, ld, old_logits, ld_old, w, N, A, out_kl, part);
   else if (G == 8) B200RL_LAUNCH(ppo_kl_cat_partial_kernel<8>, nb, 256, 0, st, logits, ld, old_logits, ld_old, w, N, A, out_kl, part);

@@ -341,9 +341,6 @@ __global__ void rf_dv_kernel(const RfArgs a) {
 
 using namespace b200rl;
 
-// Lanes per logits row (as cat_group in ppo.cu).
-static int rf_group(int64_t A) { return A <= 8 ? 1 : (A <= 64 ? 8 : 32); }
-
 static int64_t rf_workspace_bytes(int64_t B, int64_t T) {
   return 4 * (kWsLast + ((B + 3) & ~3LL) + B * T);
 }
@@ -386,9 +383,8 @@ int b200rl_reinforce_loss(const float* p0, const float* p1, int64_t ld, const vo
     nb3 = (unsigned)(want > kRfLossBlocks ? kRfLossBlocks : want);
     B200RL_LAUNCH(rf_loss_normal_kernel, nb3, 256, 0, st, a);
   } else {
-    const int G = rf_group(A);
-    const int64_t want = (N * G + 255) / 256;
-    nb3 = (unsigned)(want > kRfLossBlocks ? kRfLossBlocks : want);
+    const int G = lane_group(A);
+    nb3 = group_blocks(N, G, kRfLossBlocks);
     if (G == 1) B200RL_LAUNCH(rf_loss_cat_kernel<1>, nb3, 256, 0, st, a);
     else if (G == 8) B200RL_LAUNCH(rf_loss_cat_kernel<8>, nb3, 256, 0, st, a);
     else B200RL_LAUNCH(rf_loss_cat_kernel<32>, nb3, 256, 0, st, a);

@@ -12,6 +12,7 @@ import torch
 from agents_b200 import _lib
 from agents_b200.policies import tf_policy
 from agents_b200.trajectories import policy_step
+from agents_b200.utils import nest
 
 _POLICY_SEED_TAG = 0x9E3779B97F4A7C15
 
@@ -34,6 +35,11 @@ class _Selecting(tf_policy.TFPolicy):
     _lib.call('b200rl_epsilon_greedy', _lib.ptr(q.contiguous()), _lib.ptr(mask), b, a,
               float(eps), self._seed, _lib.ptr(self._rng), None, None, _lib.ptr(out),
               _lib.stream())
+    # column j of q is action minimum + j (the reference's ShiftedCategorical)
+    spec = nest.flatten(self.action_spec)[0]
+    minimum = int(np.asarray(getattr(spec, 'minimum', 0)).reshape(-1)[0])
+    if minimum != 0:
+      out += minimum
     return out if dtype == torch.int32 else out.to(dtype)
 
 

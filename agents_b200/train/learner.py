@@ -31,7 +31,7 @@ def _agent_state_tensors(agent):
                '_value_network', '_critic_network_1', '_critic_network_2', '_target_critic_network_1',
                '_target_critic_network_2', '_target_actor_network', '_critic_network',
                '_target_critic_network', '_target_q_network_delayed',
-               '_target_q_network_delayed_2'):
+               '_target_q_network_delayed_2', '_cloning_network'):
     net = getattr(agent, name, None)
     if net is not None and hasattr(net, 'flat_params'):
       out[name] = net.flat_params
@@ -51,8 +51,9 @@ def _agent_state_tensors(agent):
   if isinstance(t, torch.Tensor):
     out['_policy/_cem_rng'] = t
   # SAC temperature; CQL-SAC's weight (a device scalar, or log_cql_alpha with Lagrange); TD3's
-  # target-smoothing Philox counter (a restored run draws the noise it would have drawn)
-  for name in ('_log_alpha', '_cql_alpha', '_log_cql_alpha', '_target_noise_rng'):
+  # target-smoothing and behavioral cloning's Normal-sample Philox counters (a restored run draws
+  # the noise it would have drawn)
+  for name in ('_log_alpha', '_cql_alpha', '_log_cql_alpha', '_target_noise_rng', '_sample_rng'):
     t = getattr(agent, name, None)
     if isinstance(t, torch.Tensor):
       out[name] = t
@@ -77,7 +78,8 @@ def _agent_state_tensors(agent):
   # buffers each agent steps, so that a freshly built agent can be restored into
   pairs = (('_optimizer', '_flat_params'), ('_critic_optimizer', '_critic_params'),
            ('_alpha_optimizer', '_log_alpha'), ('_cql_alpha_optimizer', '_log_cql_alpha'))
-  nets = (('_optimizer', '_q_network'), ('_actor_optimizer', '_actor_network'))
+  nets = (('_optimizer', '_q_network'), ('_actor_optimizer', '_actor_network'),
+          ('_optimizer', '_cloning_network'))
   for oname, pname in pairs:
     opt, p = getattr(agent, oname, None), getattr(agent, pname, None)
     if hasattr(opt, '_get_slots') and isinstance(p, torch.Tensor):

@@ -535,6 +535,41 @@ int b200rl_epsilon_uniform(float* action, int64_t ld, int64_t N, int64_t A, floa
                            uint64_t* rng_call_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * Behavioral cloning (csrc/behavioral_cloning.cu).  Replaces the default losses of
+ * agents/behavioral_cloning/behavioral_cloning_agent.py with common.aggregate_losses and
+ * tf.math.multiply_no_nan: loss = sum_n w_n pe_n / N over N rows (B, or B*T), where a row with
+ * w_n = 0 adds exactly 0 and has an all-zero gradient even when pe_n is inf or NaN.  w_n =
+ * weights[n / w_div] (w_div = 1: per row, T: per batch entry, N: a scalar); weights may be NULL
+ * (all 1).  per_example [N] receives the unweighted pe_n.  workspace: >= 512 floats.  Two-stage
+ * fixed-order reduction.  nan_flag may be NULL; it is set when the loss is not finite.
+ * ------------------------------------------------------------------------------------ */
+/* tf.nn.sparse_softmax_cross_entropy_with_logits(labels=action - minimum, logits): logits [N, A]
+ * (row stride ld), labels action[n * action_stride] - minimum; pe_n = log sum_j exp(z_j) -
+ * z_label; dlogits [N, A] (row stride ld_g) = w_n / N (softmax - onehot(label)).  A label outside
+ * [0, A) sets nan_flag and pe_n = NaN. */
+int b200rl_bc_discrete_loss(const float* logits, int64_t ld, const int32_t* action,
+                            int64_t action_stride, int32_t minimum, const float* weights,
+                            int64_t w_div, int64_t N, int64_t A, float* loss, float* per_example,
+                            float* dlogits, int64_t ld_g, int32_t* nan_flag, void* workspace,
+                            int64_t ws_bytes, void* stream);
+/* tf.losses.mse(target, a): pe_n = mean_k (a_nk - t_nk)^2, target [N, A] with row stride ld_t.
+ * scale == NULL: pred is an ActorNetwork's tanh output y, a = 0.5 (amax + amin) + 0.5 (amax -
+ * amin) y, and dpred = 0.5 (amax - amin) 2 w_n (a - t) / (N A).
+ * scale != NULL: (pred, scale) = (loc, scale) of a Normal, a = loc + scale z (not clipped), with
+ * z = noise_in[n * A + k] or N(0, 1) by Box-Muller on the Philox block of element n * A + k of
+ * the call rng_call_dev[0] (b200rl_normal_sample's stream); dpred = dloc = 2 w_n (a - t) / (N A),
+ * dscale = dloc z.  advance_rng: the call counter advances by one after the draws.
+ * pred, scale, dpred and dscale share row strides ld (inputs) and ld_g (gradients). */
+int b200rl_bc_continuous_loss(const float* pred, const float* scale, int64_t ld,
+                              const float* target, int64_t ld_t, const float* amin,
+                              const float* amax, const float* noise_in, uint64_t seed,
+                              uint64_t* rng_call_dev, int advance_rng, const float* weights,
+                              int64_t w_div, int64_t N, int64_t A, float* loss,
+                              float* per_example, float* dpred, float* dscale, int64_t ld_g,
+                              int32_t* nan_flag, void* workspace, int64_t ws_bytes,
+                              void* stream);
+
+/* ------------------------------------------------------------------------------------
  * CQL-SAC (csrc/cql.cu).  Replaces agents/cql/cql_sac_agent.py (_cql_loss :534-679, actor_loss
  * :681-750, _get_cql_alpha :752-765, reward noise :832-839, the Lagrange step of _train
  * :336-348).  The critic joint input x is [B + 2BN, D+A]: rows [0, B) (s, a_data), [B, B+BN) the
