@@ -148,6 +148,9 @@ SIGNATURES = {
     'b200rl_dense_bwd': [_P, c_i64, _P, _P, _P, _P, _P, c_i64, c_i64, c_i64, c_int, c_int, _P, c_i64,
                          _P],
     'b200rl_act_bwd': [_P, _P, _P, c_i64, c_int, _P],
+    'b200rl_lstm_plan': [c_i64, c_i64, _P, _P, _P, _P, _P, _P, _P],
+    'b200rl_lstm_seq_fwd': [_P, _P, _P, _P, _P, c_i64, c_i64, c_i64, _P, _P, _P, _P, _P, _P, _P],
+    'b200rl_lstm_seq_bwd': [_P, _P, _P, _P, _P, _P, c_i64, c_i64, c_i64, _P, _P],
     'b200rl_conv2d_fwd': [_P, c_int, c_f32, _P, _P, _P, ctypes.POINTER(ConvGeom), c_int, _P,
                           c_i64, _P],
     'b200rl_conv2d_bwd': [_P, c_int, c_f32, _P, _P, _P, _P, _P, ctypes.POINTER(ConvGeom), c_int,

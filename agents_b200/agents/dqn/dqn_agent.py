@@ -77,6 +77,10 @@ class DqnAgent(tf_agent.TFAgent):
     net_observation_spec = time_step_spec.observation
     if self._splitter is not None:
       net_observation_spec, _ = self._splitter(net_observation_spec)
+    for net in (q_network, target_q_network):
+      if net is not None and getattr(net, 'state_spec', ()):
+        raise NotImplementedError('DqnAgent supports feed-forward Q networks only: a recurrent '
+                                  'network needs sequence training.')
     q_network.create_variables(net_observation_spec)
     if target_q_network is not None:
       target_q_network.create_variables(net_observation_spec)

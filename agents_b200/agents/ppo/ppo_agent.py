@@ -17,6 +17,11 @@ Device work of `train(experience[B, T])` (csrc/ppo.cu, scans.cu, nn.cu, optim.cu
   affine scans over T-1 steps) -> trajectory mask/weights -> behaviour log-probs -> advantage
   moments + normalisation, then per epoch: actor + value forward, fused surrogate/value/entropy
   loss with gradients, backward, global-norm scale, fused Adam on the joint flat buffer.
+A recurrent actor or value net (ActorDistributionRnnNetwork, ValueRnnNetwork) runs over the whole
+[B, T] sequence from the zero state with the step-type resets in the three network passes: the
+value pass of preprocessing, each epoch's forward and backward, and the post-epoch KL pass
+(ppo_agent.py:525-530, 981-986).  The loss kernels, GAE and the optimiser step are unchanged over
+the N = B*T rows.
 """
 import collections
 import ctypes
@@ -149,7 +154,7 @@ class PPOAgent(tf_agent.TFAgent):
       raise ValueError('Experience used for advantage calculation must have >1 num_steps.')
     dev = obs.device
     if self._compute_value_and_advantage_in_train:
-      vp, _ = self._collect_policy.apply_value_network(obs)
+      vp, _ = self._collect_policy.apply_value_network(obs, *self._seq(self._value_net, experience))
       vp = vp.reshape(B, T).contiguous()
     else:                                                         # :775-776
       vp = experience.policy_info['value_prediction'].float().reshape(B, T).contiguous()
@@ -191,10 +196,22 @@ class PPOAgent(tf_agent.TFAgent):
       out = nest.map_structure(lambda t: t.squeeze(0), out)
     return out
 
+  @property
+  def recurrent(self):
+    return bool(self._actor_net.state_spec or self._value_net.state_spec)
+
+  @staticmethod
+  def _seq(net, experience):
+    """Extra arguments of a network pass over the flattened [B, T] rows: the step types for a
+    recurrent net (its sequences start from the zero state), none for a feed-forward one."""
+    return (experience.step_type,) if net.state_spec else ()
+
   # ---- train (ppo_agent.py:834-1076) ------------------------------------------------------------
   def _train(self, experience, weights=None):
     if self._optimizer is None:
       raise ValueError('Optimizer is undefined.')
+    if self.recurrent and self.replicas > 1:
+      raise NotImplementedError('PPOAgent with a recurrent network trains on one replica.')
     if not isinstance(experience, trajectory.Trajectory):
       raise TypeError('Input type not supported: {}'.format(type(experience)))
     tf_agent.validate_trajectory(experience, self.training_data_spec, None)
@@ -267,9 +284,11 @@ class PPOAgent(tf_agent.TFAgent):
     scalars = (float(self._importance_ratio_clipping), float(self._value_clipping),
                float(self._value_pred_loss_coef), float(self._entropy_regularization),
                float(self._log_prob_clipping))
+    aseq = self._seq(self._actor_net, experience)
+    vseq = self._seq(self._value_net, experience)
     for _ in range(self._num_epochs):                             # :925-967
-      params, actx = self._actor_net.forward_train(obs_n)
-      v, vtape = self._value_net.forward_train(obs_n)
+      params, actx = self._actor_net.forward_train(obs_n, *aseq)
+      v, vtape = self._value_net.forward_train(obs_n, *vseq)
       if use_kl:
         self._mean_kl(params, old_params, w, N, A, n_glob)
         self._kl_penalty_terms()
@@ -302,7 +321,9 @@ class PPOAgent(tf_agent.TFAgent):
       self._optimizer.apply_flat(self._flat_params, self._flat_grads, scale_dev)
       self._bump_train_step(1)
     if self._initial_adaptive_kl_beta > 0:                        # :978-989
-      params = self._actor_net.distribution_params(obs_n)
+      params = self._actor_net.distribution_params(obs_n, *aseq)
+      if aseq:
+        params = params[0]                                        # (params, final state)
       self._mean_kl(params, old_params, w, N, A, n_glob)
       self._update_beta()
     if self.update_normalizers_in_train:                          # :991-993
@@ -400,13 +421,17 @@ class PPOAgent(tf_agent.TFAgent):
       if not coef:
         continue
       for l in net.layers:
-        k = getattr(l, 'kernel', None)
-        if k is None:
+        if getattr(l, 'kernel', None) is None:
           continue
-        _lib.call('b200rl_l2_sum', _lib.ptr(k), k.numel(), float(coef) / self.replicas,
-                  _lib.ptr(l2_accum), _lib.stream())
-        _lib.call('b200rl_add_scaled', _lib.ptr(l.d_kernel), _lib.ptr(k), k.numel(),
-                  2.0 * float(coef) / self.replicas, _lib.stream())
+        # every variable named '*kernel*' (:1097-1103): an LSTM's recurrent_kernel too
+        pairs = [(l.kernel, l.d_kernel)]
+        if getattr(l, 'recurrent_kernel', None) is not None:
+          pairs.append((l.recurrent_kernel, l.d_recurrent_kernel))
+        for k, dk in pairs:
+          _lib.call('b200rl_l2_sum', _lib.ptr(k), k.numel(), float(coef) / self.replicas,
+                    _lib.ptr(l2_accum), _lib.stream())
+          _lib.call('b200rl_add_scaled', _lib.ptr(dk), _lib.ptr(k), k.numel(),
+                    2.0 * float(coef) / self.replicas, _lib.stream())
 
   def update_observation_normalizer(self, batched_observations):
     if self._observation_normalizer is not None:

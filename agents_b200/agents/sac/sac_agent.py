@@ -93,6 +93,11 @@ class SacAgent(tf_agent.TFAgent):
                initial_log_alpha=0.0, use_log_alpha_in_alpha_loss=True, target_entropy=None,
                gradient_clipping=None, debug_summaries=False, summarize_grads_and_vars=False,
                train_step_counter=None, name=None, seed=0):
+    for net in (critic_network, actor_network, critic_network_2, target_critic_network,
+                target_critic_network_2):
+      if net is not None and getattr(net, 'state_spec', ()):
+        raise NotImplementedError('SacAgent supports feed-forward networks only: a recurrent '
+                                  'network needs sequence training.')
     flat_action_spec = nest.flatten(action_spec)
     if len(flat_action_spec) != 1:
       raise NotImplementedError('Only a single continuous action tensor is supported.')

@@ -94,6 +94,36 @@ def encoder_layers(preprocessing_layers, conv_layer_params, fc_layer_params, act
   return layers
 
 
+def normal_head_fwd(m_raw, std_bias, amin, amax):
+  """(loc, scale) [N, A] of the NormalProjectionNetwork head from the mean layer's output."""
+  n, a = m_raw.shape
+  loc = torch.empty_like(m_raw)
+  scale = torch.empty_like(m_raw)
+  _lib.call('b200rl_normal_proj_fwd', _lib.ptr(m_raw), _lib.ptr(std_bias), _lib.ptr(amin),
+            _lib.ptr(amax), n, a, _lib.ptr(loc), _lib.ptr(scale), _lib.stream())
+  return loc, scale
+
+
+def normal_head_bwd(m_raw, std_bias, amin, amax, dparams):
+  """(dm_raw, per-row std-bias gradient) from dparams = (dloc, dscale), each [N, A]."""
+  dloc, dscale = dparams
+  n, a = m_raw.shape
+  dm = torch.empty_like(m_raw)
+  ds_part = torch.empty_like(m_raw)
+  _lib.call('b200rl_normal_proj_bwd', _lib.ptr(m_raw), _lib.ptr(std_bias), _lib.ptr(amin),
+            _lib.ptr(amax), _lib.ptr(dloc), _lib.ptr(dscale), n, a, _lib.ptr(dm),
+            _lib.ptr(ds_part), _lib.stream())
+  return dm, ds_part
+
+
+def reduce_std_grad(ds_part, d_std_bias):
+  """d_std_bias <- column sums of the per-row std-bias gradient."""
+  n, a = ds_part.shape
+  ws, nb = workspace.get(ds_part.device)
+  _lib.call('b200rl_colsum', _lib.ptr(ds_part), None, 0, n, a, 1.0, _lib.ptr(d_std_bias),
+            _lib.ptr(ws), nb, _lib.stream())
+
+
 class ActorDistributionNetwork(network.Network):
   """Emits the parameters of the action distribution: (loc, scale) of a diagonal Normal over
   bounded continuous actions, or the [N, A] logits of a Categorical over discrete ones."""
@@ -153,13 +183,7 @@ class ActorDistributionNetwork(network.Network):
     return self._amax
 
   def _head(self, m_raw):
-    n = m_raw.shape[0]
-    loc = torch.empty_like(m_raw)
-    scale = torch.empty_like(m_raw)
-    _lib.call('b200rl_normal_proj_fwd', _lib.ptr(m_raw), _lib.ptr(self._std.bias),
-              _lib.ptr(self._amin), _lib.ptr(self._amax), n, self.num_actions, _lib.ptr(loc),
-              _lib.ptr(scale), _lib.stream())
-    return loc, scale
+    return normal_head_fwd(m_raw, self._std.bias, self._amin, self._amax)
 
   def distribution_params(self, observation):
     """(loc, scale) each [N, A], or logits [N, A] for a discrete action; no tape."""
@@ -180,17 +204,9 @@ class ActorDistributionNetwork(network.Network):
     if self.discrete:
       return super().backward(ctx, dparams)
     tape, m_raw = ctx
-    dloc, dscale = dparams
-    n = m_raw.shape[0]
-    dm = torch.empty_like(m_raw)
-    ds_part = torch.empty_like(m_raw)
-    _lib.call('b200rl_normal_proj_bwd', _lib.ptr(m_raw), _lib.ptr(self._std.bias),
-              _lib.ptr(self._amin), _lib.ptr(self._amax), _lib.ptr(dloc), _lib.ptr(dscale), n,
-              self.num_actions, _lib.ptr(dm), _lib.ptr(ds_part), _lib.stream())
+    dm, ds_part = normal_head_bwd(m_raw, self._std.bias, self._amin, self._amax, dparams)
     grads = super().backward(tape, dm)      # zeroes the flat gradient, then accumulates
-    ws, nb = workspace.get(m_raw.device)
-    _lib.call('b200rl_colsum', _lib.ptr(ds_part), None, 0, n, self.num_actions, 1.0,
-              _lib.ptr(self._std.d_bias), _lib.ptr(ws), nb, _lib.stream())
+    reduce_std_grad(ds_part, self._std.d_bias)
     return grads
 
   def __call__(self, observation, step_type=None, network_state=(), training=False):

@@ -24,12 +24,14 @@ _ACTOR_SEED_TAG = 0x4143544F52504F4C
 class ActorPolicy(tf_policy.TFPolicy):
 
   _SEED_TAG = _ACTOR_SEED_TAG
+  _STATEFUL_ACTOR = False        # subclasses that thread a recurrent actor's state set True
 
   def __init__(self, time_step_spec, action_spec, actor_network, clip=True, collect=True, seed=0,
-               info_spec=()):
-    if getattr(actor_network, 'state_spec', ()):
+               info_spec=(), policy_state_spec=()):
+    if getattr(actor_network, 'state_spec', ()) and not self._STATEFUL_ACTOR:
       raise NotImplementedError('ActorPolicy supports stateless actor networks only.')
-    super().__init__(time_step_spec, action_spec, info_spec=info_spec)
+    super().__init__(time_step_spec, action_spec, policy_state_spec=policy_state_spec,
+                     info_spec=info_spec)
     self._actor_net = actor_network
     self._clip, self._collect = clip, collect
     self._seed = (int(seed) ^ self._SEED_TAG) & 0xFFFFFFFFFFFFFFFF

@@ -59,6 +59,8 @@ class PPOLearner(object):
                use_kwargs_in_agent_train=False, strategy=None, seed=0):
     if minibatch_size and shuffle_buffer_size is None:
       raise ValueError('shuffle_buffer_size must be provided if minibatch_size is not None.')
+    if minibatch_size and getattr(agent, 'recurrent', False):        # ppo_learner.py:174-177
+      raise ValueError('minibatch_size must be set to None for RNN networks.')
     if minibatch_size and agent._compute_value_and_advantage_in_train:
       raise ValueError('agent.compute_value_and_advantage_in_train should be set to False '
                        'when mini batching is used.')

@@ -658,6 +658,29 @@ int b200rl_dense_bwd(const float* X, int64_t ldx, const float* W, const float* d
 int b200rl_act_bwd(const float* Y, const float* dY, float* dZ, int64_t n, int act,
                    void* stream);
 
+/* LSTM sequence recurrence (keras LSTMCell, implementation=2, under DynamicUnroll:
+ * keras_layers/dynamic_unroll_layer.py; csrc/lstm.cu).  Gate columns i, f, g, o; U is the
+ * [H, 4H] recurrent kernel; step_type [B, T] (FIRST = 0 resets the state to zero).  1 <= H <= 256.
+ * b200rl_lstm_seq_fwd: xw [B, T, 4H] = x W + b (from b200rl_dense_fwd); h0 / c0 [B, H] optional
+ * (NULL = zeros).  Writes h [B, T, H], the post-activation gates [B, T, 4H], c [B, T, H],
+ * h_used [B, T, H] (the h_{t-1} each step consumed: zero at a reset, so dU = h_used^T dG) and the
+ * final state hT / cT [B, H] (optional).  One launch runs all T steps.
+ * b200rl_lstm_seq_bwd: reverse-time pass from dh [B, T, H] and the stored forward values to the
+ * pre-activation gate gradients dG [B, T, 4H]; no gradient crosses a reset step or reaches h0 / c0
+ * (c0 is read for the forget-gate gradient of step 0).  U must be 16-byte aligned.
+ * b200rl_lstm_plan: the launch shapes of the two kernels for (B, H): the cluster size (shared),
+ * batch rows per cluster, cp.async ring depths and shared memory per CTA of each (the backward
+ * takes fewer rows where its dG buffers leave no room for more; any output may be NULL). */
+int b200rl_lstm_plan(int64_t B, int64_t H, int* cluster, int* rows_fwd, int* rows_bwd,
+                     int* depth_fwd, int* depth_bwd, int64_t* smem_fwd, int64_t* smem_bwd);
+int b200rl_lstm_seq_fwd(const float* xw, const float* U, const int32_t* step_type,
+                        const float* h0, const float* c0, int64_t B, int64_t T, int64_t H,
+                        float* h, float* gates, float* c, float* h_used, float* hT, float* cT,
+                        void* stream);
+int b200rl_lstm_seq_bwd(const float* dh, const float* gates, const float* c, const float* c0,
+                        const float* U, const int32_t* step_type, int64_t B, int64_t T,
+                        int64_t H, float* dG, void* stream);
+
 /* conv2d, NHWC, VALID padding, square stride.  X is [N,H,W,C] f32, or u8 when x_is_u8
  * (then each element is converted to f32 and DIVIDED by x_scale — the reference's
  * cast+/255 preprocessing layer, examples/dqn/mnih15/dqn_train_eval_atari.py:104).
