@@ -71,6 +71,14 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
 #define B200RL_LAUNCH(kernel, grid, block, smem, st, ...) \
   (void)::b200rl::launch_k(kernel, dim3(grid), dim3(block), (size_t)(smem), st, __VA_ARGS__)
 
+// 256-thread blocks for n elements, one element per thread.
+static inline unsigned blocks_of_256(int64_t n) { return (unsigned)((n + 255) / 256); }
+
+// Width of a one-block reduction over n elements: n rounded up to whole warps, at most 1024.
+static inline unsigned reduce_threads(int64_t n) {
+  return n >= 1024 ? 1024u : (unsigned)((n + 31) / 32 * 32);
+}
+
 // ---- Philox4x32-10 (Salmon et al. 2011), the counter-based generator of this library -----
 // counter = (elem_lo, elem_hi, call_lo, call_hi), key = (seed_lo, seed_hi).
 // oracle/philox.py restates exactly this; tests/test_philox.py pins both against the
@@ -124,19 +132,47 @@ __device__ __forceinline__ float philox_normal(uint64_t elem, uint64_t call, uin
   return sqrtf(-2.f * logf(u1)) * cospif(2.f * uniform_f32(r.y));
 }
 
-// The last block to finish advances the Philox call counter {call, ticket} (as sac_sample), so a
+// ---- last-block-done ticket -----------------------------------------------------------------
+// The device-resident counters (Philox call index, replay last_id, optimiser step, Periodically
+// counter) are advanced once per launch by the last block of the grid to finish, so a captured
+// graph sees the new value on every replay.  One thread per block calls this after a
+// __syncthreads() that follows the block's last read of the counters.  It returns true in exactly
+// one block, with the ticket already back at 0; that block then stores the counters and calls
+// __threadfence().  The ticket counts every block of the grid, whatever its shape.
+__device__ __forceinline__ bool last_block_ticket(uint32_t* ticket) {
+  __threadfence();
+  const unsigned int tk = atomicAdd(ticket, 1u);
+  if (tk != gridDim.x * gridDim.y * gridDim.z - 1) return false;
+  *ticket = 0u;
+  return true;
+}
+
+// Advances the Philox call counter rng_call = uint64[2] {call, ticket} once per launch, so a
 // captured graph draws fresh values on every replay.  Every thread of the grid must reach it, and
 // every block must have read rng_call[0] before.
 __device__ __forceinline__ void next_rng_call(uint64_t* rng_call) {
   __syncthreads();
-  if (threadIdx.x == 0) {
+  if (threadIdx.x == 0 && last_block_ticket((uint32_t*)(rng_call + 1))) {
+    rng_call[0] = rng_call[0] + 1;
     __threadfence();
-    unsigned int tk = atomicAdd((uint32_t*)(rng_call + 1), 1u);
-    if (tk == gridDim.x - 1) {
-      *(uint32_t*)(rng_call + 1) = 0u;
-      rng_call[0] = rng_call[0] + 1;
-      __threadfence();
-    }
+  }
+}
+
+// ---- TD element loss (td3.cu, ddpg.cu, qtopt.cu) ------------------------------------------------
+// l = l(e) + l0 and g = dl/dq for the TD error e = y - q.  Huber (delta 1): l(e) = 0.5 e^2 for
+// |e| <= 1 else |e| - 0.5, dl/dq = -clip(e, -1, 1); squared: l(e) = e^2, dl/dq = -2e.
+// l0 takes a second critic's loss, so the twin-critic squared sum is fma(e1, e1, e2^2).  The
+// default l0 = -0 is the exact additive identity (x + -0 = x and fma(e, e, -0) = e * e for
+// every x and e).
+__device__ __forceinline__ void td_elem_loss(float e, int kind, float& l, float& g,
+                                             float l0 = -0.f) {
+  if (kind == B200RL_LOSS_HUBER) {
+    const float a = fabsf(e);
+    l = (a <= 1.f ? 0.5f * e * e : a - 0.5f) + l0;
+    g = -fminf(fmaxf(e, -1.f), 1.f);
+  } else {
+    l = fmaf(e, e, l0);
+    g = -2.f * e;
   }
 }
 

@@ -65,14 +65,7 @@ __global__ void cql_reward_noise_kernel(const float* __restrict__ reward, int64_
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < B) {
     const float s = stddev[0];
-    float z;
-    if (z_in) {
-      z = z_in[i];
-    } else {
-      const Philox4 r = philox4x32_10((uint64_t)i, rng_call[0], seed);
-      const float u1 = ((float)(r.x >> 8) + 1.0f) * (1.0f / 16777216.0f);
-      z = sqrtf(-2.f * logf(u1)) * cospif(2.f * uniform_f32(r.y));
-    }
+    const float z = z_in ? z_in[i] : philox_normal((uint64_t)i, rng_call[0], seed);
     out[i] = s > 0.f ? __fadd_rn(reward[i], __fmul_rn(z, s)) : reward[i];
   }
   if (!z_in) next_rng_call(rng_call);
@@ -262,8 +255,6 @@ __global__ void cql_bc_actor_bwd_kernel(const float* __restrict__ head,
 
 using namespace b200rl;
 
-static unsigned cql_blocks(int64_t n) { return (unsigned)((n + 255) / 256); }
-
 extern "C" {
 
 int b200rl_cql_candidates(const float* obs, int64_t ld_obs, int64_t B, int64_t N, int64_t D,
@@ -275,7 +266,7 @@ int b200rl_cql_candidates(const float* obs, int64_t ld_obs, int64_t B, int64_t N
                    "cql_candidates: bad argument");
   B200RL_CHECK_ARG(u_in || rng_call_dev, "cql_candidates: need u_in or rng_call_dev");
   const int64_t n = 2 * B * N * (D + A) + B * N * 2 * A;
-  B200RL_LAUNCH(cql_candidates_kernel, cql_blocks(n), 256, 0, (cudaStream_t)stream, obs, ld_obs, B, N, D, A, amin, amax, u_in, seed, rng_call_dev, head, x, head_tiled);
+  B200RL_LAUNCH(cql_candidates_kernel, blocks_of_256(n), 256, 0, (cudaStream_t)stream, obs, ld_obs, B, N, D, A, amin, amax, u_in, seed, rng_call_dev, head, x, head_tiled);
   B200RL_CHECK_LAUNCH("cql_candidates");
   return B200RL_OK;
 }
@@ -285,7 +276,7 @@ int b200rl_cql_reward_noise(const float* reward, int64_t B, const float* stddev_
                             void* stream) {
   B200RL_CHECK_ARG(reward && stddev_dev && out && B >= 1, "cql_reward_noise: bad argument");
   B200RL_CHECK_ARG(z_in || rng_call_dev, "cql_reward_noise: need z_in or rng_call_dev");
-  B200RL_LAUNCH(cql_reward_noise_kernel, cql_blocks(B), 256, 0, (cudaStream_t)stream, reward, B, stddev_dev, z_in, seed, rng_call_dev, out);
+  B200RL_LAUNCH(cql_reward_noise_kernel, blocks_of_256(B), 256, 0, (cudaStream_t)stream, reward, B, stddev_dev, z_in, seed, rng_call_dev, out);
   B200RL_CHECK_LAUNCH("cql_reward_noise");
   return B200RL_OK;
 }
@@ -344,7 +335,7 @@ int b200rl_cql_bc_actor_bwd(const float* head, const float* action, int64_t ld_a
   B200RL_CHECK_ARG(head && action && amin && amax && train_step_dev && dhead && B >= 1 &&
                        A >= 1 && ld_action >= A && global_batch > 0.f,
                    "cql_bc_actor_bwd: bad argument");
-  B200RL_LAUNCH(cql_bc_actor_bwd_kernel, cql_blocks(B * A), 256, 0, (cudaStream_t)stream, head, action, ld_action, amin, amax, weights, train_step_dev, num_bc_steps, B, A, loss_weight, global_batch, dhead);
+  B200RL_LAUNCH(cql_bc_actor_bwd_kernel, blocks_of_256(B * A), 256, 0, (cudaStream_t)stream, head, action, ld_action, amin, amax, weights, train_step_dev, num_bc_steps, B, A, loss_weight, global_batch, dhead);
   B200RL_CHECK_LAUNCH("cql_bc_actor_bwd");
   return B200RL_OK;
 }

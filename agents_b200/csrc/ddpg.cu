@@ -13,9 +13,8 @@
 
 namespace b200rl {
 
-// y = reward_scale r + gamma d tq;  loss = sum_b w_b l(y, q_b) / B;  dq_b = w_b / B * dl/dq_b.
-// Huber (delta 1): l = 0.5 e^2 for |e| <= 1 else |e| - 0.5, dl/dq = -clip(e, -1, 1); squared:
-// l = e^2, dl/dq = -2e; e = y - q.
+// y = reward_scale r + gamma d tq;  loss = sum_b w_b l(y, q_b) / B;  dq_b = w_b / B * dl/dq_b,
+// l = td_elem_loss of e = y - q.
 __global__ void __launch_bounds__(1024) ddpg_critic_loss_kernel(
     const float* __restrict__ q, const float* __restrict__ tq, const float* __restrict__ reward,
     const float* __restrict__ discount, const float* __restrict__ weights, int64_t B,
@@ -30,14 +29,7 @@ __global__ void __launch_bounds__(1024) ddpg_critic_loss_kernel(
     if (td_targets) td_targets[b] = y;
     const float e = y - q[b];
     float l, g;
-    if (loss_kind == B200RL_LOSS_HUBER) {
-      const float a = fabsf(e);
-      l = a <= 1.f ? 0.5f * e * e : a - 0.5f;
-      g = -fminf(fmaxf(e, -1.f), 1.f);
-    } else {
-      l = e * e;
-      g = -2.f * e;
-    }
+    td_elem_loss(e, loss_kind, l, g);
     const float w = weights ? weights[b] : 1.f;
     s += l * w;
     dq[b] = g * (w * inv_b);
@@ -78,19 +70,12 @@ __global__ void __launch_bounds__(1024) ddpg_actor_loss_kernel(
   }
 }
 
-// The OU step of component k: (1 - damping) x_k + stddev z_k, with z_k = noise_in[k] or Philox +
-// Box-Muller on element k of the call rng_call[0].  Every thread that needs x_new[k] computes it
-// from the unchanged x_old, so every block sees the same value.
+// The OU step of component k: (1 - damping) x_k + stddev z_k, with z_k = noise_in[k] or
+// philox_normal on element k of the call rng_call[0].  Every thread that needs x_new[k] computes
+// it from the unchanged x_old, so every block sees the same value.
 __device__ __forceinline__ float ou_step(const float* state, int64_t k, float rho, float stddev,
                                          const float* noise_in, uint64_t seed, uint64_t call) {
-  float z;
-  if (noise_in) {
-    z = noise_in[k];
-  } else {
-    const Philox4 r = philox4x32_10((uint64_t)k, call, seed);
-    const float u1 = ((float)(r.x >> 8) + 1.0f) * (1.0f / 16777216.0f);  // (0,1]
-    z = sqrtf(-2.f * logf(u1)) * cospif(2.f * uniform_f32(r.y));
-  }
+  const float z = noise_in ? noise_in[k] : philox_normal((uint64_t)k, call, seed);
   return __fmaf_rn(rho, state[k], stddev * z);
 }
 
@@ -115,11 +100,7 @@ __global__ void ou_noise_kernel(const float* __restrict__ loc, int64_t ld_loc, i
     out[n * ld_out + k] = v;
   }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const unsigned int tk = atomicAdd((uint32_t*)(rng_call + 1), 1u);
-    last = tk == gridDim.x - 1;
-  }
+  if (threadIdx.x == 0) last = last_block_ticket((uint32_t*)(rng_call + 1));
   __syncthreads();
   if (!last) return;
   __threadfence();
@@ -127,7 +108,6 @@ __global__ void ou_noise_kernel(const float* __restrict__ loc, int64_t ld_loc, i
     state[k] = ou_step(state, k, rho, stddev, noise_in, seed, call);
   __syncthreads();
   if (threadIdx.x == 0) {
-    *(uint32_t*)(rng_call + 1) = 0u;
     if (!noise_in) rng_call[0] = call + 1;
     __threadfence();
   }
@@ -136,10 +116,6 @@ __global__ void ou_noise_kernel(const float* __restrict__ loc, int64_t ld_loc, i
 }  // namespace b200rl
 
 using namespace b200rl;
-
-static unsigned ddpg_reduce_threads(int64_t n) {
-  return n >= 1024 ? 1024u : (unsigned)((n + 31) / 32 * 32);
-}
 
 extern "C" {
 
@@ -151,7 +127,7 @@ int b200rl_ddpg_critic_loss(const float* q, const float* tq, const float* reward
                    "ddpg_critic_loss: bad argument");
   B200RL_CHECK_ARG(loss_kind == B200RL_LOSS_HUBER || loss_kind == B200RL_LOSS_SQUARED,
                    "ddpg_critic_loss: unknown loss kind");
-  B200RL_LAUNCH(ddpg_critic_loss_kernel, 1, ddpg_reduce_threads(B), 0, (cudaStream_t)stream, q, tq, reward, discount, weights, B, gamma, reward_scale, loss_kind, loss, dq, td_targets, nan_flag);
+  B200RL_LAUNCH(ddpg_critic_loss_kernel, 1, reduce_threads(B), 0, (cudaStream_t)stream, q, tq, reward, discount, weights, B, gamma, reward_scale, loss_kind, loss, dq, td_targets, nan_flag);
   B200RL_CHECK_LAUNCH("ddpg_critic_loss");
   return B200RL_OK;
 }
@@ -163,7 +139,7 @@ int b200rl_ddpg_actor_loss(const float* dqda, int64_t ld_dqda, const float* weig
   B200RL_CHECK_ARG(dqda && amin && amax && loss && dy && B >= 1 && A >= 1 && ld_dqda >= A,
                    "ddpg_actor_loss: bad argument");
   B200RL_CHECK_ARG(!clip || dqda_clipping >= 0.f, "ddpg_actor_loss: negative dqda_clipping");
-  B200RL_LAUNCH(ddpg_actor_loss_kernel, 1, ddpg_reduce_threads(B * A), 0, (cudaStream_t)stream, dqda, ld_dqda, weights, B, A, clip, dqda_clipping, amin, amax, loss, dy, nan_flag);
+  B200RL_LAUNCH(ddpg_actor_loss_kernel, 1, reduce_threads(B * A), 0, (cudaStream_t)stream, dqda, ld_dqda, weights, B, A, clip, dqda_clipping, amin, amax, loss, dy, nan_flag);
   B200RL_CHECK_LAUNCH("ddpg_actor_loss");
   return B200RL_OK;
 }

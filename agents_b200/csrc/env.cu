@@ -14,19 +14,6 @@ namespace b200rl {
 constexpr int kFirst = 0, kMid = 1, kLast = 2;   // trajectories/time_step.py:113-121
 constexpr uint64_t kStateDomain = 1ull << 62;    // Philox element index domain for per-env draws
 
-__device__ __forceinline__ void bump_call(uint64_t* rng_call, uint32_t* ticket_word) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    unsigned int tk = atomicAdd(ticket_word, 1u);
-    if (tk == gridDim.x * gridDim.y - 1) {
-      *ticket_word = 0u;
-      rng_call[0] = rng_call[0] + 1;
-      __threadfence();
-    }
-  }
-}
-
 // rng_call layout: uint64[2] = {call index, ticket (low 32 bits used)}.
 __global__ void __launch_bounds__(256) eps_greedy_kernel(const float* __restrict__ q,
                                                          const int32_t* __restrict__ mask,
@@ -70,7 +57,7 @@ __global__ void __launch_bounds__(256) eps_greedy_kernel(const float* __restrict
     }
     out[b] = (u >= eps) ? best : rnd;  // tf.where(rng >= epsilon, greedy, random)
   }
-  if (!u_in) bump_call(rng_call, (uint32_t*)(rng_call + 1));
+  if (!u_in) next_rng_call(rng_call);
 }
 
 // grid = (chunks, B).  Each thread fills 16 B of observation from one Philox block.
@@ -118,7 +105,7 @@ __global__ void __launch_bounds__(256) env_random_step_kernel(
     step_type[b] = nst;
     if (out_step_type) out_step_type[b] = nst;
   }
-  bump_call(rng_call, (uint32_t*)(rng_call + 1));
+  next_rng_call(rng_call);
 }
 
 __global__ void __launch_bounds__(256) env_cartpole_step_kernel(
@@ -165,7 +152,7 @@ __global__ void __launch_bounds__(256) env_cartpole_step_kernel(
     state[b * 4 + 0] = x; state[b * 4 + 1] = xd; state[b * 4 + 2] = th; state[b * 4 + 3] = thd;
     obs[b * 4 + 0] = x; obs[b * 4 + 1] = xd; obs[b * 4 + 2] = th; obs[b * 4 + 3] = thd;
   }
-  bump_call(rng_call, (uint32_t*)(rng_call + 1));
+  next_rng_call(rng_call);
 }
 
 }  // namespace b200rl

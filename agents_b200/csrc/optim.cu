@@ -3,27 +3,15 @@
 // buffer, so each of these is a single HBM-bound launch:
 //   Adam   28 B/param (read g,m,v,p; write m,v,p)     Polyak 12 B/param
 // The reference issues one assign op per variable (utils/common.py:328-331) and leaves the
-// optimiser to TensorFlow (agents/dqn/dqn_agent.py:444).  Counters live on the device and are
-// advanced by the last block to finish, so the launches are CUDA-graph replayable.
+// optimiser to TensorFlow (agents/dqn/dqn_agent.py:444).  Counters live on the device as
+// int64[2] {value, ticket} and are advanced by the last block to finish, so the launches are
+// CUDA-graph replayable.  last_block_ticket uses the low 32-bit word of the ticket; the word is
+// back at 0 after every launch, so the high word stays 0.
 #include <math.h>
 
 #include "common.cuh"
 
 namespace b200rl {
-
-// counter block layout: int64[2] = {value, ticket}
-__device__ __forceinline__ void last_block_store(int64_t* ctr, int64_t new_value) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    unsigned long long tk = atomicAdd((unsigned long long*)(ctr + 1), 1ull);
-    if (tk == (unsigned long long)gridDim.x - 1) {
-      ctr[1] = 0;
-      ctr[0] = new_value;
-      __threadfence();
-    }
-  }
-}
 
 // kGated: every block returns before touching anything unless *gate % gate_period == 0, so a
 // skipped update leaves p, m, v and the step counter as they were.
@@ -56,7 +44,11 @@ __global__ void __launch_bounds__(256) adam_tf_kernel(float* __restrict__ p,
     v[i] = vi;
     p[i] = p[i] - (mi * lr_t) / (sqrtf(vi) + eps);
   }
-  last_block_store(step, t);
+  __syncthreads();
+  if (threadIdx.x == 0 && last_block_ticket((uint32_t*)(step + 1))) {
+    step[0] = t;
+    __threadfence();
+  }
 }
 
 __device__ __forceinline__ void rmsprop_one(float& p, float g, float& ms, float* mg, float& mom,
@@ -131,7 +123,13 @@ __global__ void __launch_bounds__(256) soft_update_kernel(float* __restrict__ ta
       else target[i] = (1.f - tau) * target[i] + tau * source[i];  // utils/common.py:328-331
     }
   }
-  if (period > 1) last_block_store(counter, c);
+  if (period > 1) {
+    __syncthreads();
+    if (threadIdx.x == 0 && last_block_ticket((uint32_t*)(counter + 1))) {
+      counter[0] = c;
+      __threadfence();
+    }
+  }
 }
 
 __global__ void __launch_bounds__(1024) clip_by_norm_segments_kernel(float* __restrict__ g,

@@ -177,8 +177,8 @@ __global__ void normal_logp_kernel(const float* __restrict__ loc, const float* _
   out[n] = logp;
 }
 
-// action = clip(loc + scale * z), z ~ N(0,1) by Box-Muller on two 24-bit uniforms of the Philox
-// block of element n*A+k; rng_call: uint64[2] {call, ticket}.
+// action = clip(loc + scale * z), z = philox_normal of element n*A+k;
+// rng_call: uint64[2] {call, ticket}.
 __global__ void normal_sample_kernel(const float* __restrict__ loc,
                                      const float* __restrict__ scale, int64_t ld, int64_t N,
                                      int64_t A, const float* __restrict__ amin,
@@ -188,24 +188,12 @@ __global__ void normal_sample_kernel(const float* __restrict__ loc,
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < N * A) {
     const int64_t n = i / A, k = i - n * A;
-    const Philox4 r = philox4x32_10((uint64_t)i, rng_call[0], seed);
-    const float u1 = ((float)(r.x >> 8) + 1.0f) * (1.0f / 16777216.0f);  // (0,1]
-    const float u2 = uniform_f32(r.y);
-    const float z = sqrtf(-2.f * logf(u1)) * cospif(2.f * u2);
+    const float z = philox_normal((uint64_t)i, rng_call[0], seed);
     float v = loc[n * ld + k] + scale[n * ld + k] * z;
     if (amin) v = fminf(fmaxf(v, amin[k]), amax[k]);
     out[i] = v;
   }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    unsigned int tk = atomicAdd((uint32_t*)(rng_call + 1), 1u);
-    if (tk == gridDim.x - 1) {
-      *(uint32_t*)(rng_call + 1) = 0u;
-      rng_call[0] = rng_call[0] + 1;
-      __threadfence();
-    }
-  }
+  next_rng_call(rng_call);
 }
 
 // NormalProjectionNetwork head (networks/normal_projection_network.py): loc = tanh-squash of
@@ -594,23 +582,12 @@ __global__ void categorical_sample_kernel(const float* __restrict__ logits, int6
     }
     out[n] = pick;
   }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    unsigned int tk = atomicAdd((uint32_t*)(rng_call + 1), 1u);
-    if (tk == gridDim.x - 1) {
-      *(uint32_t*)(rng_call + 1) = 0u;
-      rng_call[0] = rng_call[0] + 1;
-      __threadfence();
-    }
-  }
+  next_rng_call(rng_call);
 }
 
 }  // namespace b200rl
 
 using namespace b200rl;
-
-static unsigned blocks_for(int64_t n) { return (unsigned)((n + 255) / 256); }
 
 extern "C" {
 
@@ -688,7 +665,7 @@ int b200rl_normal_logp(const float* loc, const float* scale, int64_t ld, const f
   B200RL_CHECK_ARG(loc && scale && action && out && N >= 0 && A >= 1 && ld >= A,
                    "normal_logp: bad argument");
   if (N == 0) return B200RL_OK;
-  B200RL_LAUNCH(normal_logp_kernel, blocks_for(N), 256, 0, (cudaStream_t)stream, loc, scale, ld, action, N, A, out);
+  B200RL_LAUNCH(normal_logp_kernel, blocks_of_256(N), 256, 0, (cudaStream_t)stream, loc, scale, ld, action, N, A, out);
   B200RL_CHECK_LAUNCH("normal_logp");
   return B200RL_OK;
 }
@@ -699,7 +676,7 @@ int b200rl_normal_sample(const float* loc, const float* scale, int64_t ld, int64
   B200RL_CHECK_ARG(loc && scale && out && rng_call_dev && N >= 1 && A >= 1 && ld >= A,
                    "normal_sample: bad argument");
   B200RL_CHECK_ARG((amin == nullptr) == (amax == nullptr), "normal_sample: amin/amax mismatch");
-  B200RL_LAUNCH(normal_sample_kernel, blocks_for(N * A), 256, 0, (cudaStream_t)stream, loc, scale, ld, N, A, amin, amax, seed, rng_call_dev, out);
+  B200RL_LAUNCH(normal_sample_kernel, blocks_of_256(N * A), 256, 0, (cudaStream_t)stream, loc, scale, ld, N, A, amin, amax, seed, rng_call_dev, out);
   B200RL_CHECK_LAUNCH("normal_sample");
   return B200RL_OK;
 }
@@ -789,7 +766,7 @@ int b200rl_categorical_sample(const float* logits, int64_t ld, int64_t N, int64_
                               uint64_t seed, uint64_t* rng_call_dev, int32_t* out, void* stream) {
   B200RL_CHECK_ARG(logits && out && rng_call_dev && N >= 1 && A >= 1 && ld >= A,
                    "categorical_sample: bad argument");
-  B200RL_LAUNCH(categorical_sample_kernel, blocks_for(N), 256, 0, (cudaStream_t)stream, logits, ld, N, A, seed, rng_call_dev, out);
+  B200RL_LAUNCH(categorical_sample_kernel, blocks_of_256(N), 256, 0, (cudaStream_t)stream, logits, ld, N, A, seed, rng_call_dev, out);
   B200RL_CHECK_LAUNCH("categorical_sample");
   return B200RL_OK;
 }
@@ -799,7 +776,7 @@ int b200rl_normal_proj_fwd(const float* m_raw, const float* s_raw, const float* 
                            void* stream) {
   B200RL_CHECK_ARG(m_raw && s_raw && amin && amax && loc && scale && N >= 1 && A >= 1,
                    "normal_proj_fwd: bad argument");
-  B200RL_LAUNCH(normal_proj_fwd_kernel, blocks_for(N * A), 256, 0, (cudaStream_t)stream, m_raw, s_raw, amin, amax, N, A, loc, scale);
+  B200RL_LAUNCH(normal_proj_fwd_kernel, blocks_of_256(N * A), 256, 0, (cudaStream_t)stream, m_raw, s_raw, amin, amax, N, A, loc, scale);
   B200RL_CHECK_LAUNCH("normal_proj_fwd");
   return B200RL_OK;
 }
@@ -810,7 +787,7 @@ int b200rl_normal_proj_bwd(const float* m_raw, const float* s_raw, const float* 
   B200RL_CHECK_ARG(m_raw && s_raw && amin && amax && dloc && dscale && dm_raw && ds_part &&
                        N >= 1 && A >= 1,
                    "normal_proj_bwd: bad argument");
-  B200RL_LAUNCH(normal_proj_bwd_kernel, blocks_for(N * A), 256, 0, (cudaStream_t)stream, m_raw, s_raw, amin, amax, dloc, dscale, N, A, dm_raw, ds_part);
+  B200RL_LAUNCH(normal_proj_bwd_kernel, blocks_of_256(N * A), 256, 0, (cudaStream_t)stream, m_raw, s_raw, amin, amax, dloc, dscale, N, A, dm_raw, ds_part);
   B200RL_CHECK_LAUNCH("normal_proj_bwd");
   return B200RL_OK;
 }
@@ -829,7 +806,7 @@ int b200rl_colsum(const float* x, const float* center, int squared, int64_t rows
   dim3 grid((unsigned)cols, (unsigned)nblk);
   B200RL_LAUNCH(colsum_rows_kernel, grid, 256, 0, st, x, center, squared, rows, cols, (float*)workspace);
   B200RL_CHECK_LAUNCH("colsum_rows");
-  B200RL_LAUNCH(colsum_rows_final_kernel, blocks_for(cols), 256, 0, st, (const float*)workspace, nblk, cols, scale, out);
+  B200RL_LAUNCH(colsum_rows_final_kernel, blocks_of_256(cols), 256, 0, st, (const float*)workspace, nblk, cols, scale, out);
   B200RL_CHECK_LAUNCH("colsum_rows_final");
   return B200RL_OK;
 }
@@ -837,7 +814,7 @@ int b200rl_colsum(const float* x, const float* center, int squared, int64_t rows
 int b200rl_normalize(const float* x, float* out, int64_t rows, int64_t cols, const float* mean,
                      const float* m2, const float* count, float eps, float clip, void* stream) {
   B200RL_CHECK_ARG(x && out && m2 && rows >= 1 && cols >= 1, "normalize: bad argument");
-  B200RL_LAUNCH(normalize_kernel, blocks_for(rows * cols), 256, 0, (cudaStream_t)stream, x, out, rows, cols, mean, m2, count, eps, clip);
+  B200RL_LAUNCH(normalize_kernel, blocks_of_256(rows * cols), 256, 0, (cudaStream_t)stream, x, out, rows, cols, mean, m2, count, eps, clip);
   B200RL_CHECK_LAUNCH("normalize");
   return B200RL_OK;
 }
@@ -847,7 +824,7 @@ int b200rl_normalizer_update(float* count, float* avg, float* m2, float* carry,
                              void* stream) {
   B200RL_CHECK_ARG(count && avg && m2 && carry && avg_a && m2_a && cols >= 1,
                    "normalizer_update: bad argument");
-  B200RL_LAUNCH(normalizer_update_kernel, blocks_for(cols), 256, 0, (cudaStream_t)stream, count, avg, m2, carry, avg_a, m2_a, n_a, cols);
+  B200RL_LAUNCH(normalizer_update_kernel, blocks_of_256(cols), 256, 0, (cudaStream_t)stream, count, avg, m2, carry, avg_a, m2_a, n_a, cols);
   B200RL_CHECK_LAUNCH("normalizer_update");
   return B200RL_OK;
 }
@@ -855,7 +832,7 @@ int b200rl_normalizer_update(float* count, float* avg, float* m2, float* carry,
 int b200rl_ppo_discounts(const float* discount, const int32_t* next_step_type, float gamma,
                          int64_t n, float* out, void* stream) {
   B200RL_CHECK_ARG(discount && next_step_type && out && n >= 1, "ppo_discounts: bad argument");
-  B200RL_LAUNCH(ppo_discounts_kernel, blocks_for(n), 256, 0, (cudaStream_t)stream, discount, next_step_type, gamma, n, out);
+  B200RL_LAUNCH(ppo_discounts_kernel, blocks_of_256(n), 256, 0, (cudaStream_t)stream, discount, next_step_type, gamma, n, out);
   B200RL_CHECK_LAUNCH("ppo_discounts");
   return B200RL_OK;
 }
@@ -863,7 +840,7 @@ int b200rl_ppo_discounts(const float* discount, const int32_t* next_step_type, f
 int b200rl_ppo_weights(const int32_t* step_type, const float* ret, const float* adv,
                        const float* weights, int64_t n, float* out, void* stream) {
   B200RL_CHECK_ARG(step_type && ret && adv && out && n >= 1, "ppo_weights: bad argument");
-  B200RL_LAUNCH(ppo_weights_kernel, blocks_for(n), 256, 0, (cudaStream_t)stream, step_type, ret, adv, weights, n, out);
+  B200RL_LAUNCH(ppo_weights_kernel, blocks_of_256(n), 256, 0, (cudaStream_t)stream, step_type, ret, adv, weights, n, out);
   B200RL_CHECK_LAUNCH("ppo_weights");
   return B200RL_OK;
 }

@@ -172,14 +172,7 @@ __global__ void __launch_bounds__(1024) qtopt_td_loss_kernel(
     const float m = step_type[b * step_stride] == 2 ? 0.f : 1.f;
     const float e = y - q[b];
     float l, g;
-    if (loss_kind == B200RL_LOSS_HUBER) {
-      const float a = fabsf(e);
-      l = a <= 1.f ? 0.5f * e * e : a - 0.5f;
-      g = -fminf(fmaxf(e, -1.f), 1.f);
-    } else {
-      l = e * e;
-      g = -2.f * e;
-    }
+    td_elem_loss(e, loss_kind, l, g);
     const float w = weights ? weights[b] : 1.f;
     td_error[b] = m * e;
     td_loss[b] = m * l;
@@ -219,8 +212,6 @@ __global__ void epsilon_uniform_kernel(float* __restrict__ action, int64_t ld, i
 
 using namespace b200rl;
 
-static unsigned qt_blocks(int64_t n) { return (unsigned)((n + 255) / 256); }
-
 extern "C" {
 
 int b200rl_cem_sample(const float* src, int64_t ld_src, int64_t B, int64_t N, int64_t C,
@@ -234,7 +225,7 @@ int b200rl_cem_sample(const float* src, int64_t ld_src, int64_t B, int64_t N, in
                    "cem_sample: bad argument");
   B200RL_CHECK_ARG(z_in || rng_call_dev, "cem_sample: need z_in or rng_call_dev");
   B200RL_CHECK_ARG(minimal_var >= 0.f, "cem_sample: negative minimal_var");
-  B200RL_LAUNCH(cem_sample_kernel, qt_blocks(B * N * (C + A)), 256, 0, (cudaStream_t)stream, src, ld_src, B, N, C, A, mean, ld_mean, var, ld_var, minimal_var, amin, amax, z_in, seed, rng_call_dev, x, ld_x);
+  B200RL_LAUNCH(cem_sample_kernel, blocks_of_256(B * N * (C + A)), 256, 0, (cudaStream_t)stream, src, ld_src, B, N, C, A, mean, ld_mean, var, ld_var, minimal_var, amin, amax, z_in, seed, rng_call_dev, x, ld_x);
   B200RL_CHECK_LAUNCH("cem_sample");
   return B200RL_OK;
 }
@@ -271,8 +262,7 @@ int b200rl_qtopt_td_loss(const float* q, const float* tq1, const float* tq2, con
                    "qtopt_td_loss: bad argument");
   B200RL_CHECK_ARG(loss_kind == B200RL_LOSS_HUBER || loss_kind == B200RL_LOSS_SQUARED,
                    "qtopt_td_loss: unknown loss kind");
-  const unsigned threads = B >= 1024 ? 1024u : (unsigned)((B + 31) / 32 * 32);
-  B200RL_LAUNCH(qtopt_td_loss_kernel, 1, threads, 0, (cudaStream_t)stream, q, tq1, tq2, reward, discount, step_type, step_stride, weights, B, gamma, reward_scale, loss_kind, loss, td_loss, td_error, dq, nan_flag);
+  B200RL_LAUNCH(qtopt_td_loss_kernel, 1, reduce_threads(B), 0, (cudaStream_t)stream, q, tq1, tq2, reward, discount, step_type, step_stride, weights, B, gamma, reward_scale, loss_kind, loss, td_loss, td_error, dq, nan_flag);
   B200RL_CHECK_LAUNCH("qtopt_td_loss");
   return B200RL_OK;
 }
@@ -282,7 +272,7 @@ int b200rl_epsilon_uniform(float* action, int64_t ld, int64_t N, int64_t A, floa
                            uint64_t* rng_call_dev, void* stream) {
   B200RL_CHECK_ARG(action && amin && amax && rng_call_dev && N >= 1 && A >= 1 && ld >= A,
                    "epsilon_uniform: bad argument");
-  B200RL_LAUNCH(epsilon_uniform_kernel, qt_blocks(N * A), 256, 0, (cudaStream_t)stream, action, ld, N, A, epsilon, amin, amax, seed, rng_call_dev);
+  B200RL_LAUNCH(epsilon_uniform_kernel, blocks_of_256(N * A), 256, 0, (cudaStream_t)stream, action, ld, N, A, epsilon, amin, amax, seed, rng_call_dev);
   B200RL_CHECK_LAUNCH("epsilon_uniform");
   return B200RL_OK;
 }

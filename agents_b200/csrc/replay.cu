@@ -187,18 +187,13 @@ template <int MODE>
 __device__ __forceinline__ void finish(const Plan& p, int64_t last, bool ok) {
   // last-block-done: advance the device-resident counters exactly once per launch.
   __syncthreads();
-  if (threadIdx.x == 0 && p.ticket != nullptr) {
-    __threadfence();
-    unsigned int tk = atomicAdd(p.ticket, 1u);
-    if (tk == gridDim.x - 1) {
-      *p.ticket = 0u;
-      if (MODE == MODE_SAMPLE) {
-        if (p.rng_call && p.ids == nullptr) *p.rng_call = *p.rng_call + 1;
-        if (p.status) *p.status = ok ? 0 : 1;
-      }
-      if (MODE == MODE_ADD) *p.last_id = last + 1;
-      __threadfence();
+  if (threadIdx.x == 0 && p.ticket != nullptr && last_block_ticket(p.ticket)) {
+    if (MODE == MODE_SAMPLE) {
+      if (p.rng_call && p.ids == nullptr) *p.rng_call = *p.rng_call + 1;
+      if (p.status) *p.status = ok ? 0 : 1;
     }
+    if (MODE == MODE_ADD) *p.last_id = last + 1;
+    __threadfence();
   }
 }
 
@@ -330,14 +325,9 @@ __global__ void draw_kernel(const __grid_constant__ Plan p) {
     p.out_draw_offs[b] = uniform_i64(r.z, r.w, 0, p.B_env);
   }
   __syncthreads();
-  if (threadIdx.x == 0) {
+  if (threadIdx.x == 0 && last_block_ticket(p.ticket)) {
+    *p.rng_call = *p.rng_call + 1;
     __threadfence();
-    unsigned int tk = atomicAdd(p.ticket, 1u);
-    if (tk == gridDim.x - 1) {
-      *p.ticket = 0u;
-      *p.rng_call = *p.rng_call + 1;
-      __threadfence();
-    }
   }
 }
 

@@ -25,14 +25,8 @@ __global__ void sac_sample_kernel(const float* __restrict__ head, int64_t N, int
   if (n < N) {
     float lp = 0.f;
     for (int64_t k = 0; k < A; ++k) {
-      float e;
-      if (eps_in) {
-        e = eps_in[n * A + k];
-      } else {
-        const Philox4 r = philox4x32_10((uint64_t)(n * A + k), rng_call[0], seed);
-        const float u1 = ((float)(r.x >> 8) + 1.0f) * (1.0f / 16777216.0f);
-        e = sqrtf(-2.f * logf(u1)) * cospif(2.f * uniform_f32(r.y));
-      }
+      const float e = eps_in ? eps_in[n * A + k]
+                             : philox_normal((uint64_t)(n * A + k), rng_call[0], seed);
       const float loc = head[n * 2 * A + k], ls = head[n * 2 * A + A + k];
       const float u = loc + expf(ls) * e;
       const float half = 0.5f * (amax[k] - amin[k]), shift = 0.5f * (amax[k] + amin[k]);
@@ -44,18 +38,7 @@ __global__ void sac_sample_kernel(const float* __restrict__ head, int64_t N, int
     }
     logp[n] = lp;
   }
-  if (!eps_in) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence();
-      unsigned int tk = atomicAdd((uint32_t*)(rng_call + 1), 1u);
-      if (tk == gridDim.x - 1) {
-        *(uint32_t*)(rng_call + 1) = 0u;
-        rng_call[0] = rng_call[0] + 1;
-        __threadfence();
-      }
-    }
-  }
+  if (!eps_in) next_rng_call(rng_call);
 }
 
 // Given dL/da (sum of up to two [N, ld] views) and dL/dlogp, write dL/dhead [N, 2A].
@@ -185,8 +168,6 @@ __global__ void concat2_kernel(const float* __restrict__ a, int64_t lda, int64_t
 
 using namespace b200rl;
 
-static unsigned sac_blocks(int64_t n) { return (unsigned)((n + 255) / 256); }
-
 extern "C" {
 
 int b200rl_sac_sample(const float* head, int64_t N, int64_t A, const float* amin,
@@ -196,7 +177,7 @@ int b200rl_sac_sample(const float* head, int64_t N, int64_t A, const float* amin
   B200RL_CHECK_ARG(head && amin && amax && action && logp && N >= 1 && A >= 1 && ld_action >= A,
                    "sac_sample: bad argument");
   B200RL_CHECK_ARG(eps_in || rng_call_dev, "sac_sample: need eps or rng_call_dev");
-  B200RL_LAUNCH(sac_sample_kernel, sac_blocks(N), 256, 0, (cudaStream_t)stream, head, N, A, amin, amax, eps_in, seed, rng_call_dev, action, ld_action, logp, u_out, eps_out);
+  B200RL_LAUNCH(sac_sample_kernel, blocks_of_256(N), 256, 0, (cudaStream_t)stream, head, N, A, amin, amax, eps_in, seed, rng_call_dev, action, ld_action, logp, u_out, eps_out);
   B200RL_CHECK_LAUNCH("sac_sample");
   return B200RL_OK;
 }
@@ -208,7 +189,7 @@ int b200rl_sac_sample_bwd(const float* head, const float* u_saved, const float* 
   B200RL_CHECK_ARG(head && u_saved && eps_saved && amin && amax && dlogp && dhead && N >= 1 &&
                        A >= 1,
                    "sac_sample_bwd: bad argument");
-  B200RL_LAUNCH(sac_sample_bwd_kernel, sac_blocks(N * A), 256, 0, (cudaStream_t)stream, head, u_saved, eps_saved, amin, amax, da1, da2, ld_da, dlogp, N, A, dhead);
+  B200RL_LAUNCH(sac_sample_bwd_kernel, blocks_of_256(N * A), 256, 0, (cudaStream_t)stream, head, u_saved, eps_saved, amin, amax, da1, da2, ld_da, dlogp, N, A, dhead);
   B200RL_CHECK_LAUNCH("sac_sample_bwd");
   return B200RL_OK;
 }
@@ -254,7 +235,7 @@ int b200rl_concat2(const float* a, int64_t lda, int64_t da, const float* b, int6
                    int64_t db, int64_t N, float* out, void* stream) {
   B200RL_CHECK_ARG(a && b && out && N >= 1 && da >= 1 && db >= 1 && lda >= da && ldb >= db,
                    "concat2: bad argument");
-  B200RL_LAUNCH(concat2_kernel, sac_blocks(N * (da + db)), 256, 0, (cudaStream_t)stream, a, lda, da, b, ldb, db, N, out);
+  B200RL_LAUNCH(concat2_kernel, blocks_of_256(N * (da + db)), 256, 0, (cudaStream_t)stream, a, lda, da, b, ldb, db, N, out);
   B200RL_CHECK_LAUNCH("concat2");
   return B200RL_OK;
 }

@@ -13,7 +13,7 @@
 namespace b200rl {
 
 // out[n, k] = mean_k + mag_k * y[n, k]  (+ clip(std * z, +-noise_clip))  (clamped to the spec).
-// z ~ N(0,1) comes from noise_in [N, A] or from Philox + Box-Muller on element n*A+k of the call
+// z ~ N(0,1) comes from noise_in [N, A] or from philox_normal on element n*A+k of the call
 // rng_call[0]; rng_call: uint64[2] {call, ticket}, advanced only when the device draws.
 // y and out may alias (the agent rewrites the action columns of a critic input in place), so
 // neither is __restrict__.
@@ -31,36 +31,17 @@ __global__ void td3_scale_to_spec_kernel(const float* y, int64_t ld_y, int64_t N
     const float lo = amin[k], hi = amax[k];
     float v = 0.5f * (hi + lo) + 0.5f * (hi - lo) * y[n * ld_y + k];
     if (noise_std > 0.f) {
-      float z;
-      if (noise_in) {
-        z = noise_in[i];
-      } else {
-        const Philox4 r = philox4x32_10((uint64_t)i, rng_call[0], seed);
-        const float u1 = ((float)(r.x >> 8) + 1.0f) * (1.0f / 16777216.0f);  // (0,1]
-        z = sqrtf(-2.f * logf(u1)) * cospif(2.f * uniform_f32(r.y));
-      }
+      const float z = noise_in ? noise_in[i] : philox_normal((uint64_t)i, rng_call[0], seed);
       v += fminf(fmaxf(noise_std * z, -noise_clip), noise_clip);
     }
     if (clamp) v = fminf(fmaxf(v, lo), hi);
     out[n * ld_out + k] = v;
   }
-  if (draw) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence();
-      unsigned int tk = atomicAdd((uint32_t*)(rng_call + 1), 1u);
-      if (tk == gridDim.x - 1) {
-        *(uint32_t*)(rng_call + 1) = 0u;
-        rng_call[0] = rng_call[0] + 1;
-        __threadfence();
-      }
-    }
-  }
+  if (draw) next_rng_call(rng_call);
 }
 
 // y = reward_scale r + gamma d min(tq1, tq2);  loss = sum_b w_b (l(y, q1) + l(y, q2)) / B;
-// dq_i = w_b / B * dl(y, q_i)/dq_i.  Huber (delta 1): l = 0.5 e^2 for |e| <= 1 else |e| - 0.5,
-// dl/dq = -clip(e, -1, 1); squared: l = e^2, dl/dq = -2e; e = y - q.
+// dq_i = w_b / B * dl(y, q_i)/dq_i, l = td_elem_loss of e = y - q.
 __global__ void __launch_bounds__(1024) td3_critic_loss_kernel(
     const float* __restrict__ q1, const float* __restrict__ q2, const float* __restrict__ tq1,
     const float* __restrict__ tq2, const float* __restrict__ reward,
@@ -76,17 +57,9 @@ __global__ void __launch_bounds__(1024) td3_critic_loss_kernel(
     const float y = reward_scale * reward[b] + gamma * discount[b] * fminf(tq1[b], tq2[b]);
     if (td_targets) td_targets[b] = y;
     const float e1 = y - q1[b], e2 = y - q2[b];
-    float l, g1, g2;
-    if (loss_kind == B200RL_LOSS_HUBER) {
-      const float a1 = fabsf(e1), a2 = fabsf(e2);
-      l = (a1 <= 1.f ? 0.5f * e1 * e1 : a1 - 0.5f) + (a2 <= 1.f ? 0.5f * e2 * e2 : a2 - 0.5f);
-      g1 = -fminf(fmaxf(e1, -1.f), 1.f);
-      g2 = -fminf(fmaxf(e2, -1.f), 1.f);
-    } else {
-      l = e1 * e1 + e2 * e2;
-      g1 = -2.f * e1;
-      g2 = -2.f * e2;
-    }
+    float l2, l, g1, g2;
+    td_elem_loss(e2, loss_kind, l2, g2);
+    td_elem_loss(e1, loss_kind, l, g1, l2);                 // l = l(e1) + l(e2)
     const float w = weights ? weights[b] : 1.f;
     s += l * w;
     const float c = w * inv_b;
@@ -139,12 +112,6 @@ __global__ void td3_actor_bwd_kernel(const float* __restrict__ da, int64_t ld_da
 
 using namespace b200rl;
 
-static unsigned td3_blocks(int64_t n) { return (unsigned)((n + 255) / 256); }
-
-static unsigned td3_reduce_threads(int64_t B) {
-  return B >= 1024 ? 1024u : (unsigned)((B + 31) / 32 * 32);
-}
-
 extern "C" {
 
 int b200rl_td3_scale_to_spec(const float* y, int64_t ld_y, int64_t N, int64_t A,
@@ -157,7 +124,7 @@ int b200rl_td3_scale_to_spec(const float* y, int64_t ld_y, int64_t N, int64_t A,
   B200RL_CHECK_ARG(noise_std >= 0.f && noise_clip >= 0.f, "td3_scale_to_spec: negative noise");
   B200RL_CHECK_ARG(noise_std == 0.f || noise_in || rng_call_dev,
                    "td3_scale_to_spec: noise needs noise_in or rng_call_dev");
-  B200RL_LAUNCH(td3_scale_to_spec_kernel, td3_blocks(N * A), 256, 0, (cudaStream_t)stream, y, ld_y, N, A, amin, amax, noise_std, noise_clip, noise_in, seed, rng_call_dev, clamp, out, ld_out);
+  B200RL_LAUNCH(td3_scale_to_spec_kernel, blocks_of_256(N * A), 256, 0, (cudaStream_t)stream, y, ld_y, N, A, amin, amax, noise_std, noise_clip, noise_in, seed, rng_call_dev, clamp, out, ld_out);
   B200RL_CHECK_LAUNCH("td3_scale_to_spec");
   return B200RL_OK;
 }
@@ -171,7 +138,7 @@ int b200rl_td3_critic_loss(const float* q1, const float* q2, const float* tq1, c
                    "td3_critic_loss: bad argument");
   B200RL_CHECK_ARG(loss_kind == B200RL_LOSS_HUBER || loss_kind == B200RL_LOSS_SQUARED,
                    "td3_critic_loss: unknown loss kind");
-  B200RL_LAUNCH(td3_critic_loss_kernel, 1, td3_reduce_threads(B), 0, (cudaStream_t)stream, q1, q2, tq1, tq2, reward, discount, weights, B, gamma, reward_scale, loss_kind, loss, dq1, dq2, td_targets, nan_flag);
+  B200RL_LAUNCH(td3_critic_loss_kernel, 1, reduce_threads(B), 0, (cudaStream_t)stream, q1, q2, tq1, tq2, reward, discount, weights, B, gamma, reward_scale, loss_kind, loss, dq1, dq2, td_targets, nan_flag);
   B200RL_CHECK_LAUNCH("td3_critic_loss");
   return B200RL_OK;
 }
@@ -179,7 +146,7 @@ int b200rl_td3_critic_loss(const float* q1, const float* q2, const float* tq1, c
 int b200rl_td3_actor_loss(const float* q, const float* weights, int64_t B, float* loss,
                           float* dq, int32_t* nan_flag, void* stream) {
   B200RL_CHECK_ARG(q && loss && dq && B >= 1, "td3_actor_loss: bad argument");
-  B200RL_LAUNCH(td3_actor_loss_kernel, 1, td3_reduce_threads(B), 0, (cudaStream_t)stream, q, weights, B, loss, dq, nan_flag);
+  B200RL_LAUNCH(td3_actor_loss_kernel, 1, reduce_threads(B), 0, (cudaStream_t)stream, q, weights, B, loss, dq, nan_flag);
   B200RL_CHECK_LAUNCH("td3_actor_loss");
   return B200RL_OK;
 }
@@ -188,7 +155,7 @@ int b200rl_td3_actor_bwd(const float* da, int64_t ld_da, const float* amin, cons
                          int64_t N, int64_t A, float* dy, void* stream) {
   B200RL_CHECK_ARG(da && amin && amax && dy && N >= 1 && A >= 1 && ld_da >= A,
                    "td3_actor_bwd: bad argument");
-  B200RL_LAUNCH(td3_actor_bwd_kernel, td3_blocks(N * A), 256, 0, (cudaStream_t)stream, da, ld_da, amin, amax, N, A, dy);
+  B200RL_LAUNCH(td3_actor_bwd_kernel, blocks_of_256(N * A), 256, 0, (cudaStream_t)stream, da, ld_da, amin, amax, N, A, dy);
   B200RL_CHECK_LAUNCH("td3_actor_bwd");
   return B200RL_OK;
 }

@@ -124,6 +124,7 @@ def test_random_env_step_bit_exact(cuda, obs_elems, u8):
     np.testing.assert_array_equal(disc.cpu().numpy(), wdisc)
     seen_last |= bool((wst == 2).any())
   assert seen_last and (wst == 0).sum() < B
+  assert rngs.cpu().tolist() == [12, 0]     # 2-D grid: one advance per launch, ticket back to 0
 
 
 def test_cartpole_step_parity(cuda):
@@ -151,3 +152,20 @@ def test_cartpole_step_parity(cuda):
     wstate, wst = state.cpu().numpy(), got_st
     assert ((disc.cpu().numpy() == wdisc) | near).all()
   assert (wsteps <= 25).all()
+  assert rngs.cpu().tolist() == [60, 0]
+  # several blocks: the resets draw from the launch's call, which advances once per launch
+  B = 600
+  state = torch.zeros(B, 4, device=cuda); steps = torch.zeros(B, dtype=torch.int32, device=cuda)
+  st = torch.full((B,), 2, dtype=torch.int32, device=cuda)
+  tact = torch.zeros(B, dtype=torch.int32, device=cuda)
+  obs = torch.empty(B, 4, device=cuda); rew = torch.empty(B, device=cuda); disc = torch.empty(B, device=cuda)
+  rngs = torch.zeros(2, dtype=torch.int64, device=cuda)
+  for call in range(2):
+    _lib.call('b200rl_env_cartpole_step', _lib.ptr(state), _lib.ptr(steps), _lib.ptr(st),
+              _lib.ptr(tact), _lib.ptr(obs), _lib.ptr(rew), _lib.ptr(disc), B, 25,
+              11, _lib.ptr(rngs), _lib.stream())
+    assert rngs.cpu().tolist() == [call + 1, 0]
+    if call == 0:
+      wstate = oenv.cartpole_step(np.zeros((B, 4), f32), np.zeros(B, np.int32), np.full(B, 2, np.int32),
+                                  np.zeros(B, np.int32), 25, 11, 0)[0]
+      np.testing.assert_allclose(state.cpu().numpy(), wstate, rtol=1e-5, atol=1e-6)

@@ -272,6 +272,12 @@ def test_custom_table_fn_uses_generic_path(cuda):
   np.testing.assert_array_equal(info.ids.cpu().numpy(), want_ids)
   np.testing.assert_array_equal(info.probabilities.cpu().numpy(), want_p)
   np.testing.assert_array_equal(rb.gather_all().cpu().numpy(), orc.gather_all()[0])
+  # a draw over several blocks advances the call once and returns the ticket to 0
+  (want,), want_ids, _, _ = orc.get_next(600, 2)
+  got, info = rb.get_next(sample_batch_size=600, num_steps=2)
+  np.testing.assert_array_equal(got.cpu().numpy(), want)
+  np.testing.assert_array_equal(info.ids.cpu().numpy(), want_ids)
+  assert int(rb._ctrl[0].item()) == orc.rng_call == 2 and int(rb._ctrl[2].item()) == 0
 
 
 def test_full_size_properties(cuda):
