@@ -14,6 +14,7 @@ LIB_PATH = os.environ.get('B200RL_LIB') or os.path.join(_HERE, 'lib', 'libb200rl
 MAX_LEAVES = 24
 ACT_NONE, ACT_RELU, ACT_TANH = 0, 1, 2
 LOSS_HUBER, LOSS_SQUARED = 0, 1
+DQN_SEQ_MAX_BLOCKS = 1024   # B200RL_DQN_SEQ_MAX_BLOCKS: partials of b200rl_dqn_seq_td_loss
 
 c_void_p = ctypes.c_void_p
 c_i64 = ctypes.c_int64
@@ -139,6 +140,9 @@ SIGNATURES = {
     'b200rl_nstep_reduce': [_P, _P, c_f64, _P, _P, c_i64, c_i64, _P],
     'b200rl_dqn_td_loss': [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_i64, c_i64, c_i64, c_i64, c_i64,
                            c_f64, c_f64, c_int, c_f32, _P, _P, _P, _P, _P, _P],
+    'b200rl_dqn_seq_td_loss': [_P, _P, _P, _P, _P, c_i64, c_i64, _P, c_i64, c_i64, _P, _P, _P,
+                               c_i64, c_i64, c_i64, c_i64, c_f64, c_f64, c_int, c_f32, _P, _P, _P,
+                               _P, _P, _P, _P, _P],
     'b200rl_c51_loss': [_P, _P, _P, _P, c_i64, _P, _P, _P, _P, c_i64, c_i64, c_i64, c_i64, c_f32,
                         c_f32, c_f32, _P, _P, _P, _P, c_i64, _P],
     'b200rl_c51_q_values': [_P, _P, c_i64, c_i64, c_i64, _P, _P],

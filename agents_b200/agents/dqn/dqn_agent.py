@@ -13,6 +13,14 @@ Device work per train step (all libb200rl, csrc/{nn,dqn,optim}.cu):
   -> Periodically-gated Polyak/hard target update                     (b200rl_soft_update)
 The reference evaluates the target network twice (:622 and inside the greedy policy :634);
 both evaluations are identical, so it is evaluated once here.
+
+With a recurrent q_network (QRnnNetwork, any LSTMEncodingNetwork) the agent trains on whole
+[B, T] sequences, T >= 2 (train_sequence_length None, dqn_agent.py:264-299): transition t of a
+sequence is (observation[:, t], action[:, t], reward[:, t], discount[:, t], observation[:, t+1])
+(trajectory.to_transition).  The online network runs over observation[:, :-1] with
+step_type[:, :-1], the target (and, for DDQN / D3QN, the online selector) over observation[:, 1:]
+with next_step_type[:, :-1], each from the zero state; b200rl_dqn_seq_td_loss then forms the
+[B, T-1] TD loss, sums it over time and aggregates it, and LSTMEncodingNetwork.backward runs BPTT.
 """
 import collections
 
@@ -77,11 +85,18 @@ class DqnAgent(tf_agent.TFAgent):
     net_observation_spec = time_step_spec.observation
     if self._splitter is not None:
       net_observation_spec, _ = self._splitter(net_observation_spec)
-    for net in (q_network, target_q_network):
-      if net is not None and getattr(net, 'state_spec', ()):
-        raise NotImplementedError('DqnAgent supports feed-forward Q networks only: a recurrent '
-                                  'network needs sequence training.')
-    q_network.create_variables(net_observation_spec)
+    self._recurrent = bool(q_network.state_spec)
+    if self._recurrent and n_step_update != 1:
+      raise NotImplementedError(
+          'DqnAgent does not currently support n-step updates with stateful '
+          'networks (i.e., RNNs), but n_step_update = {}'.format(n_step_update))
+    out = q_network.create_variables(net_observation_spec)
+    if self._recurrent and tuple(out.shape) != (self._num_actions,):
+      # e.g. a bare LSTMEncodingNetwork: an encoder, not a recurrent Q network
+      raise NotImplementedError(
+          'DqnAgent trains feed-forward Q networks and recurrent Q networks that emit ({},) Q '
+          'values per step (QRnnNetwork); this stateful q_network emits {}.'.format(
+              self._num_actions, tuple(out.shape)))
     if target_q_network is not None:
       target_q_network.create_variables(net_observation_spec)
       if target_q_network is q_network:
@@ -106,7 +121,7 @@ class DqnAgent(tf_agent.TFAgent):
                                                    device)
     self._seed = seed
     policy, collect_policy = self._setup_policy(time_step_spec, action_spec)
-    train_sequence_length = n_step_update + 1
+    train_sequence_length = None if self._recurrent else n_step_update + 1
     super(DqnAgent, self).__init__(
         time_step_spec, action_spec, policy, collect_policy,
         train_sequence_length=train_sequence_length, debug_summaries=debug_summaries,
@@ -119,6 +134,9 @@ class DqnAgent(tf_agent.TFAgent):
     self.replicas = 1           # set by train.Learner for data-parallel runs
     self._grad_sync = None      # callable(flat_grads) installed by train.Learner
     self._comm_stream = torch.cuda.Stream(device=device)
+    if self._recurrent:   # b200rl_dqn_seq_td_loss scratch: block partials and a last-block ticket
+      self._seq_partials = torch.empty(_lib.DQN_SEQ_MAX_BLOCKS, dtype=torch.float32, device=device)
+      self._seq_ticket = torch.zeros(1, dtype=torch.int32, device=device)
 
   # ---- construction helpers -----------------------------------------------------------------
   def _check_action_spec(self, action_spec):
@@ -174,8 +192,22 @@ class DqnAgent(tf_agent.TFAgent):
   def _forward_loss(self, experience, weights, keep_tape):
     exp = self._prepare(experience)
     B, T = exp.discount.shape[0], exp.discount.shape[1]
-    obs0, _ = self._split_obs(nest.map_structure(lambda t: t[:, 0], exp.observation))
-    obsn, next_mask = self._split_obs(nest.map_structure(lambda t: t[:, T - 1], exp.observation))
+    if self._recurrent:
+      if self.replicas > 1:
+        raise NotImplementedError('DqnAgent with a recurrent network trains on one replica.')
+      if T < 2:
+        raise ValueError('Trajectory frame count must be at least 2, but saw {}'.format(T))
+      # [B, T-1] sequences: the online net sees time_steps, the target side next_time_steps
+      obs0, _ = self._split_obs(nest.map_structure(lambda t: t[:, :-1], exp.observation))
+      obsn, next_mask = self._split_obs(nest.map_structure(lambda t: t[:, 1:], exp.observation))
+      if next_mask is not None:
+        next_mask = next_mask.reshape(B * (T - 1), self._num_actions)
+      online_args = (obs0, exp.step_type[:, :-1])
+      target_args = (obsn, exp.next_step_type[:, :-1])
+    else:
+      obs0, _ = self._split_obs(nest.map_structure(lambda t: t[:, 0], exp.observation))
+      obsn, next_mask = self._split_obs(nest.map_structure(lambda t: t[:, T - 1], exp.observation))
+      online_args, target_args = (obs0,), (obsn,)
     # The target-side forwards do not depend on the online forward: inside a captured graph fork
     # them onto a side stream and join before the TD kernel (eager launches are host-bound, the
     # fork only pays inside a graph).
@@ -185,24 +217,28 @@ class DqnAgent(tf_agent.TFAgent):
       side.wait_stream(main)
     with torch.cuda.stream(side if side is not None else main), \
         workspace.slot(1 if side is not None else 0):
-      next_t, _ = self._target_q_network(obsn)
+      next_t, _ = self._target_q_network(*target_args)
       if isinstance(next_t, tuple):                # dueling nets may emit (q, ...) (:723-726)
         next_t = next_t[0]
       next_sel = next_t
       if self._DOUBLE_Q:
-        next_sel, _ = self._q_network(obsn)        # DdqnAgent (dqn_agent.py:686-688)
+        next_sel, _ = self._q_network(*target_args)  # DdqnAgent (dqn_agent.py:686-688)
         if isinstance(next_sel, tuple):            # D3qnAgent reads element 1 (:730)
           next_sel = next_sel[1] if self._SELECT_UNMASKED else next_sel[0]
     if self._SELECT_UNMASKED:
       next_mask = None                             # tf.math.argmax on the raw values (:731)
     if keep_tape:
-      q, tape = self._q_network.forward_train(obs0)
+      q, tape = self._q_network.forward_train(*online_args)
     else:
-      (q, _), tape = self._q_network(obs0), None
+      (q, _), tape = self._q_network(*online_args), None
     if side is not None:
       main.wait_stream(side)
     else:
       workspace.mirror(q.device, 1)   # size the side-stream scratch for a later capture
+    if self._recurrent:
+      rows = (B * (T - 1), self._num_actions)
+      return self._td_seq(exp, B, T, q.reshape(rows), next_t.reshape(rows),
+                          next_sel.reshape(rows), next_mask, weights, tape)
     return self._td(exp, B, T, q, next_t, next_sel, next_mask, weights, tape)
 
   def _td(self, exp, B, T, q, next_t, next_sel, next_mask, weights, tape):
@@ -229,12 +265,43 @@ class DqnAgent(tf_agent.TFAgent):
               float(self._reward_scale_factor), self._loss_kind, float(B * self.replicas),
               _lib.ptr(loss), _lib.ptr(td_loss), _lib.ptr(td_error), _lib.ptr(dq),
               _lib.ptr(self._nan_flag), _lib.stream())
-    # regularisation losses (common.aggregate_losses :1470-1475)
+    return loss, td_loss, td_error, dq, tape, self._add_reg_loss(loss)
+
+  def _td_seq(self, exp, B, T, q, next_t, next_sel, next_mask, weights, tape):
+    """The [B, T-1] sequence TD loss and dLoss/dq from the three [B*(T-1), A] tables (one kernel);
+    td_loss is [B] (summed over time) and td_error [B, T-1]."""
+    dev = q.device
+    actions, a_ld, a_st = self._int32_bt(exp.action)
+    steps, s_ld, s_st = self._int32_bt(exp.step_type)
+    rew = exp.reward.float().contiguous()
+    disc = exp.discount.float().contiguous()
+    w_stride = 0
+    if weights is not None:
+      weights = torch.as_tensor(weights, dtype=torch.float32, device=dev)
+      if weights.numel() > 1:
+        weights, w_stride = weights.reshape(B).contiguous(), 1
+    if next_mask is not None:
+      next_mask = next_mask.to(torch.int32).contiguous()
+    loss = torch.empty(1, dtype=torch.float32, device=dev)
+    td_loss = torch.empty(B, dtype=torch.float32, device=dev)
+    td_error = torch.empty((B, T - 1), dtype=torch.float32, device=dev)
+    dq = torch.empty_like(q)
+    _lib.call('b200rl_dqn_seq_td_loss', _lib.ptr(q), _lib.ptr(next_t), _lib.ptr(next_sel),
+              _lib.ptr(next_mask), _lib.dptr(actions), a_ld, a_st,
+              _lib.dptr(steps), s_ld, s_st, _lib.ptr(rew), _lib.ptr(disc), _lib.ptr(weights),
+              w_stride, B, self._num_actions, T, float(self._gamma),
+              float(self._reward_scale_factor), self._loss_kind, float(B), _lib.ptr(loss),
+              _lib.ptr(td_loss), _lib.ptr(td_error), _lib.ptr(dq), _lib.ptr(self._nan_flag),
+              _lib.ptr(self._seq_partials), _lib.ptr(self._seq_ticket), _lib.stream())
+    return loss, td_loss, td_error, dq, tape, self._add_reg_loss(loss)
+
+  def _add_reg_loss(self, loss):
+    """Adds the regularisation losses to `loss` (common.aggregate_losses :1470-1475)."""
     reg = self._q_network.losses
     for coef, w in reg:
       _lib.call('b200rl_l2_sum', _lib.ptr(w), w.numel(), float(coef) / self.replicas,
                 _lib.ptr(loss), _lib.stream())
-    return loss, td_loss, td_error, dq, tape, reg
+    return reg
 
   @staticmethod
   def _column0(t):
@@ -244,6 +311,15 @@ class DqnAgent(tf_agent.TFAgent):
     if col.dtype != torch.int32:
       return col.to(torch.int32).contiguous(), 1
     return col, (col.stride(0) if col.numel() > 1 else 1)
+
+  @staticmethod
+  def _int32_bt(t):
+    """(tensor, row stride, time stride) of an int [B, T] tensor: element (b, t) is
+    tensor.data_ptr()[b * row + t * time]; int32 storage is read in place, other dtypes are cast
+    once."""
+    if t.dtype != torch.int32:
+      t = t.to(torch.int32).contiguous()
+    return t, t.stride(0), t.stride(1)
 
   def _loss(self, experience, td_errors_loss_fn=None, gamma=None, reward_scale_factor=None,
             weights=None, training=False):
@@ -274,7 +350,8 @@ class DqnAgent(tf_agent.TFAgent):
           with torch.cuda.stream(comm):
             self._grad_sync(net.flat_grads[state['lo']:state['sent']])
           state['sent'] = state['lo']
-    grads = net.backward(tape, dq, grad_hook=hook)
+    # (the recurrent backward takes no hook: bucketed is False on its one replica)
+    grads = net.backward(tape, dq, grad_hook=hook) if bucketed else net.backward(tape, dq)
     if bucketed:
       main = torch.cuda.current_stream()
       if state['sent'] > 0:

@@ -147,6 +147,16 @@ class LSTMEncodingNetwork(network.Network):
                   for n in (output_fc_layer_params or ())]
     self._layers = self._pre + self._cells + self._post
 
+  def copy(self, **kwargs):
+    """Network.copy replaces `_layers` only; the copy's encoder, cell and output lists must hold
+    the copied layers (bound to the copy's variables), not the original's."""
+    new = super().copy(**kwargs)
+    n_pre, n_cells = len(self._pre), len(self._cells)
+    new._pre = new._layers[:n_pre]
+    new._cells = new._layers[n_pre:n_pre + n_cells]
+    new._post = new._layers[n_pre + n_cells:]
+    return new
+
   # ---- state ------------------------------------------------------------------------------
   def get_initial_state(self, batch_size=None):
     return nest.map_structure(

@@ -45,7 +45,7 @@ class CategoricalQPolicy(q_policy.QPolicy):
   def support(self):
     return self._support
 
-  def q_values(self, time_step):
+  def q_values(self, time_step, policy_state=()):
     obs, mask = time_step.observation, None
     if self._splitter is not None:
       obs, mask = self._splitter(obs)
@@ -55,4 +55,4 @@ class CategoricalQPolicy(q_policy.QPolicy):
     q = torch.empty((b, self._num_actions), dtype=torch.float32, device=logits.device)
     _lib.call('b200rl_c51_q_values', _lib.ptr(logits), _lib.ptr(self._support), b,
               self._num_actions, self._num_atoms, _lib.ptr(q), _lib.stream())
-    return q, mask
+    return q, mask, policy_state

@@ -3,7 +3,9 @@
 Reference: policies/epsilon_greedy_policy.py:120-145 (`u ~ U[0, 1)` per batch row, the random
 branch is `RandomTFPolicy` over the same action mask).  Device work: one b200rl_epsilon_greedy
 launch (greedy_policy._Selecting).  `epsilon` may be a float or a callable evaluated on the host at
-every call (:93-99).
+every call (:93-99).  With a recurrent Q network the returned state is the greedy branch's new
+state on every row, including the rows that take the random action (the reference returns
+`greedy_action.state`).
 
 For a bounded float action spec (QtOptAgent's collect policy over CEMPolicy) the wrapped policy's
 action is taken and, per row with probability epsilon, replaced by a uniform draw in
@@ -23,7 +25,8 @@ class EpsilonGreedyPolicy(_Selecting):
   """where(u >= epsilon, greedy, uniform random) (epsilon_greedy_policy.py:120-145)."""
 
   def __init__(self, policy, epsilon, seed=0, name=None):
-    super().__init__(policy.time_step_spec, policy.action_spec, seed=seed, name=name)
+    super().__init__(policy.time_step_spec, policy.action_spec, seed=seed, name=name,
+                     policy_state_spec=policy.policy_state_spec)
     self._wrapped_policy = policy
     self._epsilon = epsilon
     self._warned_capture = False
@@ -41,6 +44,9 @@ class EpsilonGreedyPolicy(_Selecting):
 
   def variables(self):
     return self._wrapped_policy.variables()
+
+  def get_initial_state(self, batch_size=None):
+    return self._wrapped_policy.get_initial_state(batch_size)
 
   def _get_epsilon(self):
     if not callable(self._epsilon):
@@ -60,6 +66,6 @@ class EpsilonGreedyPolicy(_Selecting):
       step = self._wrapped_policy.action(time_step, policy_state, seed)
       act = self._float.apply(step.action.float().clone(), self._get_epsilon())
       return policy_step.PolicyStep(act, step.state, step.info)
-    q, mask = self._wrapped_policy.q_values(time_step)
+    q, mask, state = self._wrapped_policy.q_values(time_step, policy_state)
     act = self._select(q, mask, self._get_epsilon(), self._wrapped_policy._action_dtype)
-    return policy_step.PolicyStep(act, policy_state, ())
+    return policy_step.PolicyStep(act, state, ())

@@ -20,8 +20,8 @@ _POLICY_SEED_TAG = 0x9E3779B97F4A7C15
 class _Selecting(tf_policy.TFPolicy):
   """Shared launch of b200rl_epsilon_greedy for the three selection policies."""
 
-  def __init__(self, time_step_spec, action_spec, seed=0, name=None):
-    super().__init__(time_step_spec, action_spec, name=name)
+  def __init__(self, time_step_spec, action_spec, seed=0, name=None, policy_state_spec=()):
+    super().__init__(time_step_spec, action_spec, policy_state_spec=policy_state_spec, name=name)
     self._seed = (int(seed) ^ _POLICY_SEED_TAG) & 0xFFFFFFFFFFFFFFFF
     self._rng = None
 
@@ -72,10 +72,11 @@ class _FloatUniform(object):
 
 
 class GreedyPolicy(_Selecting):
-  """argmax_a Q(s,a) (greedy_policy.py:70-89)."""
+  """argmax_a Q(s,a) (greedy_policy.py:70-89).  The state is the wrapped QPolicy's."""
 
   def __init__(self, policy, name=None):
-    super().__init__(policy.time_step_spec, policy.action_spec, name=name)
+    super().__init__(policy.time_step_spec, policy.action_spec, name=name,
+                     policy_state_spec=policy.policy_state_spec)
     self._wrapped_policy = policy
 
   @property
@@ -85,7 +86,10 @@ class GreedyPolicy(_Selecting):
   def variables(self):
     return self._wrapped_policy.variables()
 
+  def get_initial_state(self, batch_size=None):
+    return self._wrapped_policy.get_initial_state(batch_size)
+
   def _action(self, time_step, policy_state, seed):
-    q, mask = self._wrapped_policy.q_values(time_step)
+    q, mask, state = self._wrapped_policy.q_values(time_step, policy_state)
     act = self._select(q, mask, -1.0, self._wrapped_policy._action_dtype)
-    return policy_step.PolicyStep(act, policy_state, ())
+    return policy_step.PolicyStep(act, state, ())

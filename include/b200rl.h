@@ -186,6 +186,34 @@ int b200rl_dqn_td_loss(const float* q, const float* next_q_tgt, const float* nex
                        float global_batch, float* loss, float* td_loss, float* td_error,
                        float* dq, int32_t* nan_flag, void* stream);
 
+/* DQN loss over the [B, T-1] transitions of a sequence (recurrent Q networks;
+ * dqn_agent.py:514-523 with trajectory.to_transition(squeeze_time_dim=False)).  Row
+ * r = b*(T-1) + t of the three tables is transition t of sequence b:
+ *   q[B*(T-1), A]            online Q over time_steps (observation[:, :-1])
+ *   next_q_tgt / next_q_sel  target Q / argmax selector over next_time_steps (observation[:, 1:])
+ *   next_mask                optional int32 [B*(T-1), A] action mask for the argmax (1 = allowed)
+ *   actions, step_type       int32, element (b, t) at ptr[b*ld + t*stride] (read in place from the
+ *                            [B, T] trajectory tensors); actions outside [0, A) are clamped and
+ *                            set *nan_flag; step LAST (2) at t masks transition t
+ *   reward, discount [B, T]  element (b, t) feeds transition t (reward[:, :-1], discount[:, :-1])
+ *   weights                  optional, weights[b*weight_stride] (0: one scalar, 1: one per row)
+ * td = reward_scale*r + gamma*d*Q_tgt(argmax Q_sel) - Q(a), DQN's Huber or squared element loss.
+ * Outputs: td_loss[B] = sum_t valid*l, td_error[B*(T-1)] = valid*td, dq[B*(T-1), A] = dLoss/dq,
+ *          loss[0] = sum_b multiply_no_nan(td_loss, w) / global_batch (no reg), nan_flag (optional
+ *          int32; set when the loss is not finite or an action was out of range).
+ * partials: >= B200RL_DQN_SEQ_MAX_BLOCKS floats of scratch; ticket: a uint32 that is 0 before the
+ * launch and is left at 0.  Fixed-order sums: repeated calls return the same bits. */
+#define B200RL_DQN_SEQ_MAX_BLOCKS 1024
+int b200rl_dqn_seq_td_loss(const float* q, const float* next_q_tgt, const float* next_q_sel,
+                           const int32_t* next_mask, const int32_t* actions, int64_t action_ld,
+                           int64_t action_stride, const int32_t* step_type, int64_t step_ld,
+                           int64_t step_stride, const float* reward, const float* discount,
+                           const float* weights, int64_t weight_stride, int64_t B, int64_t A,
+                           int64_t T, double gamma, double reward_scale, int loss_kind,
+                           float global_batch, float* loss, float* td_loss, float* td_error,
+                           float* dq, int32_t* nan_flag, float* partials, uint32_t* ticket,
+                           void* stream);
+
 /* ------------------------------------------------------------------------------------
  * Categorical DQN (C51) loss, forward + backward -- agents/categorical_dqn/
  * categorical_dqn_agent.py:271-556 (+ project_distribution :562-731).
