@@ -15,6 +15,7 @@ MAX_LEAVES = 24
 ACT_NONE, ACT_RELU, ACT_TANH = 0, 1, 2
 LOSS_HUBER, LOSS_SQUARED = 0, 1
 DQN_SEQ_MAX_BLOCKS = 1024   # B200RL_DQN_SEQ_MAX_BLOCKS: partials of b200rl_dqn_seq_td_loss
+DDPG_SEQ_MAX_BLOCKS = 1024  # B200RL_DDPG_SEQ_MAX_BLOCKS: partials of b200rl_ddpg_seq_*_loss
 
 c_void_p = ctypes.c_void_p
 c_i64 = ctypes.c_int64
@@ -115,6 +116,10 @@ SIGNATURES = {
     'b200rl_td3_actor_bwd': [_P, c_i64, _P, _P, c_i64, c_i64, _P, _P],
     'b200rl_ddpg_critic_loss': [_P, _P, _P, _P, _P, c_i64, c_f32, c_f32, c_int, _P, _P, _P, _P, _P],
     'b200rl_ddpg_actor_loss': [_P, c_i64, _P, c_i64, c_i64, c_int, c_f32, _P, _P, _P, _P, _P, _P],
+    'b200rl_ddpg_seq_critic_loss': [_P, _P, _P, _P, c_i64, c_i64, _P, c_i64, c_i64, c_i64, c_f32,
+                                    c_f32, c_int, _P, _P, _P, _P, _P, _P],
+    'b200rl_ddpg_seq_actor_loss': [_P, c_i64, _P, c_i64, c_i64, c_i64, c_i64, c_int, c_f32, _P, _P,
+                                   _P, _P, _P, _P, _P, _P],
     'b200rl_ou_noise': [_P, c_i64, c_i64, c_i64, _P, c_f32, c_f32, _P, c_u64, _P, _P, _P, _P, c_i64,
                         _P],
     'b200rl_cem_sample': [_P, c_i64, c_i64, c_i64, c_i64, c_i64, _P, c_i64, _P, c_i64, c_f32, _P,

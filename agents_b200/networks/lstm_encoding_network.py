@@ -94,8 +94,10 @@ class LSTM(L.Layer):
               _lib.stream())
     return h, (hT, cT), (x, gates, c, h_used, c0, step_type, B, T)
 
-  def backward_seq(self, ctx, dh, need_dx):
-    """Accumulates dW, dU, db into the gradient views; returns dx [B*T, in] (or None)."""
+  def backward_seq(self, ctx, dh, need_dx, need_param_grads=True):
+    """Accumulates dW, dU, db into the gradient views; returns dx [B*T, in] (or None).
+    need_param_grads=False runs only the BPTT and the dx GEMM: the gradient views are untouched
+    (DDPG's dQ/da through a recurrent critic)."""
     x, gates, c, h_used, c0, step_type, B, T = ctx
     H, dev = self.units, x.device
     n = B * T
@@ -105,13 +107,17 @@ class LSTM(L.Layer):
               _lib.ptr(self.recurrent_kernel), _lib.ptr(step_type), B, T, H, _lib.ptr(dG),
               _lib.stream())
     dx = torch.empty((n, self.in_features), dtype=torch.float32, device=dev) if need_dx else None
+    if not (need_dx or need_param_grads):
+      return None
     ws, nb = workspace.get(dev)
+    dw, db = (self.d_kernel, self.d_bias) if need_param_grads else (None, None)
     _lib.call('b200rl_dense_bwd', _lib.ptr(x), self.in_features, _lib.ptr(self.kernel),
-              _lib.ptr(dG), _lib.ptr(dx), _lib.ptr(self.d_kernel), _lib.ptr(self.d_bias), n,
+              _lib.ptr(dG), _lib.ptr(dx), _lib.ptr(dw), _lib.ptr(db), n,
               self.in_features, 4 * H, 1, _lib.ACT_NONE, _lib.ptr(ws), nb, _lib.stream())
-    _lib.call('b200rl_dense_bwd', _lib.ptr(h_used), H, _lib.ptr(self.recurrent_kernel),
-              _lib.ptr(dG), None, _lib.ptr(self.d_recurrent_kernel), None, n, H, 4 * H, 1,
-              _lib.ACT_NONE, _lib.ptr(ws), nb, _lib.stream())
+    if need_param_grads:
+      _lib.call('b200rl_dense_bwd', _lib.ptr(h_used), H, _lib.ptr(self.recurrent_kernel),
+                _lib.ptr(dG), None, _lib.ptr(self.d_recurrent_kernel), None, n, H, 4 * H, 1,
+                _lib.ACT_NONE, _lib.ptr(ws), nb, _lib.stream())
     return dx
 
 
@@ -211,14 +217,21 @@ class LSTMEncodingNetwork(network.Network):
 
   def _run_seq(self, obs, st, B, T, network_state):
     """Returns (output [B*T, ...], new_state, tape)."""
-    pre_tape, post_tape, ctxs, finals = [], [], [], []
+    pre_tape = []
     x = self._run_stack(self._pre, obs, pre_tape)
+    x, state, ctxs, post_tape = self._run_recurrent(x, st, B, T, network_state)
+    return x, state, (pre_tape, ctxs, post_tape)
+
+  def _run_recurrent(self, x, st, B, T, network_state):
+    """The LSTM layers and the output stack over the encoded rows x [B*T, ...]; returns
+    (output [B*T, ...], new_state, cell contexts, output-stack tape)."""
+    post_tape, ctxs, finals = [], [], []
     for cell, s in zip(self._cells, self._layer_states(network_state)):
       x, fin, ctx = cell.forward_seq(x, st, B, T, s)
       ctxs.append(ctx)
       finals.append(fin)
     x = self._run_stack(self._post, x, post_tape)
-    return x, self._pack_state(finals), (pre_tape, ctxs, post_tape)
+    return x, self._pack_state(finals), ctxs, post_tape
 
   def _unflatten(self, out, B, T, has_time):
     return out.reshape(((B, T) if has_time else (B,)) + tuple(out.shape[1:]))
@@ -238,14 +251,24 @@ class LSTMEncodingNetwork(network.Network):
   def backward(self, tape, dy):
     """Back-propagates dLoss/d(output [B*T, ...]) through `tape`, OVERWRITING flat_grads."""
     pre_tape, ctxs, post_tape = tape
-    if any(l.has_params for l, _, _ in post_tape):
-      _, dh = super().backward(post_tape, dy, need_input_grad=True)
-    else:
-      self._grads.zero_()
-      dh = dy
     need_pre = any(l.has_params for l, _, _ in pre_tape)
-    for i in range(len(self._cells) - 1, -1, -1):
-      dh = self._cells[i].backward_seq(ctxs[i], dh, need_dx=i > 0 or need_pre)
+    dh = self._backward_recurrent(ctxs, post_tape, dy, need_pre)
     if need_pre:
       super().backward(pre_tape, dh, zero_grads=False)
     return self._grads
+
+  def _backward_recurrent(self, ctxs, post_tape, dy, need_dx, need_param_grads=True):
+    """Back-propagates dy through the output stack and the LSTM layers of `_run_recurrent`;
+    returns dLoss/d(the first LSTM layer's input) when need_dx.  With need_param_grads the
+    gradients are OVERWRITTEN from here on; without, flat_grads is left untouched."""
+    if any(l.has_params for l, _, _ in post_tape):
+      _, dh = network.Network.backward(self, post_tape, dy, need_input_grad=True,
+                                       need_param_grads=need_param_grads)
+    else:
+      if need_param_grads:
+        self._grads.zero_()
+      dh = dy
+    for i in range(len(self._cells) - 1, -1, -1):
+      dh = self._cells[i].backward_seq(ctxs[i], dh, need_dx=i > 0 or need_dx,
+                                       need_param_grads=need_param_grads)
+    return dh

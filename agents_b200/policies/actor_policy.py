@@ -7,7 +7,10 @@ collect=True  -> a draw from the distribution: Normal(loc, scale) through b200rl
 collect=False -> the greedy policy, the mode of the distribution: loc for a Normal, the first
                  argmax of the logits for a Categorical (b200rl_epsilon_greedy with epsilon 0).
 A deterministic network (ActorNetwork, `deterministic = True`) gives its scale_to_spec action,
-clamped to the action spec when `clip`; `collect` does not apply.
+clamped to the action spec when `clip`; `collect` does not apply.  A recurrent deterministic actor
+(ActorRnnNetwork) makes the policy stateful: `policy_state_spec` is the actor's `state_spec`, and
+each call runs one [B, 1] step from the given state (the zero state where step_type is FIRST) and
+returns the new state.
 Draws use a device {call, ticket} counter, so a captured collect step draws fresh values on every
 replay.  Subclasses record extra `policy_info` through `_info` (PPOPolicy).
 """
@@ -28,8 +31,13 @@ class ActorPolicy(tf_policy.TFPolicy):
 
   def __init__(self, time_step_spec, action_spec, actor_network, clip=True, collect=True, seed=0,
                info_spec=(), policy_state_spec=()):
+    self._stateful_deterministic = False
     if getattr(actor_network, 'state_spec', ()) and not self._STATEFUL_ACTOR:
-      raise NotImplementedError('ActorPolicy supports stateless actor networks only.')
+      if not getattr(actor_network, 'deterministic', False):
+        raise NotImplementedError('ActorPolicy supports stateless actor networks and recurrent '
+                                  'deterministic actors (ActorRnnNetwork) only.')
+      self._stateful_deterministic = True
+      policy_state_spec = actor_network.state_spec
     super().__init__(time_step_spec, action_spec, policy_state_spec=policy_state_spec,
                      info_spec=info_spec)
     self._actor_net = actor_network
@@ -44,6 +52,11 @@ class ActorPolicy(tf_policy.TFPolicy):
 
   def variables(self):
     return self._actor_net.variables
+
+  def get_initial_state(self, batch_size=None):
+    if not self._stateful_deterministic:
+      return super().get_initial_state(batch_size)
+    return self._actor_net.get_initial_state(batch_size)
 
   def _normalized(self, observation):
     return observation
@@ -89,6 +102,13 @@ class ActorPolicy(tf_policy.TFPolicy):
 
   def _action(self, time_step, policy_state, seed):
     obs = self._normalized(time_step.observation)
+    if self._stateful_deterministic:
+      if len(nest.flatten(policy_state)) != len(nest.flatten(self._policy_state_spec)):
+        raise ValueError('This ActorPolicy is stateful (its actor is recurrent): pass the '
+                         'policy_state from get_initial_state(batch_size) or from the previous '
+                         'action().')
+      act, state = self._actor_net.action(obs, time_step.step_type, policy_state, clip=self._clip)
+      return policy_step.PolicyStep(act, state, self._info(obs, act))
     if getattr(self._actor_net, 'deterministic', False):
       act = self._actor_net.action(obs, clip=self._clip)
       return policy_step.PolicyStep(act, policy_state, self._info(obs, act))

@@ -3,7 +3,8 @@ Ornstein-Uhlenbeck noise (utils/common.py OUProcess), clipped to the action spec
 
 The OU state x has the unbatched action shape [A] and starts at zeros.  Each `action()` call
 advances it once, x <- (1 - ou_damping) x + N(0, ou_stddev), and adds the same x to every row of
-the batch; as in the reference the state is never reset at episode boundaries.  One
+the batch; as in the reference the state is never reset at episode boundaries.  A stateful
+wrapped policy (a recurrent actor) owns the policy state: its new state is returned as is.  One
 b200rl_ou_noise launch per call does both.  The state and the {call, ticket} Philox counter are
 device tensors allocated here, so a captured collect step advances them on every replay.
 """
@@ -53,6 +54,9 @@ class OUNoisePolicy(tf_policy.TFPolicy):
   def ou_state(self):
     """The OU process value x [A] after the last `action()` call."""
     return self._ou_state
+
+  def get_initial_state(self, batch_size=None):
+    return self._wrapped_policy.get_initial_state(batch_size)
 
   def variables(self):
     return self._wrapped_policy.variables()

@@ -504,6 +504,31 @@ int b200rl_ddpg_actor_loss(const float* dqda, int64_t ld_dqda, const float* weig
                            int64_t A, int clip, float dqda_clipping, const float* amin,
                            const float* amax, float* loss, float* dy, int32_t* nan_flag,
                            void* stream);
+/* Recurrent DDPG: the two losses over the [B, T-1] transitions of [B, T] sequences
+ * (ddpg_agent.py with data_converter.AsTransition(squeeze_time_dim=False)).  Row
+ * r = b*(T-1) + t of q, tq, dq, dqda and dy is transition t of sequence b.
+ *   reward, discount  element (b, t) at ptr[b*ld + t*stride], read in place from the [B, T]
+ *                     experience (transition t reads step t)
+ *   weights           optional, weights[b*weight_stride] (0: one scalar, 1: one per row)
+ * critic: y = reward_scale*r + gamma*d*tq; td_loss_b = sum_t l(y, q) (no LAST mask, as the
+ *   reference); loss = sum_b w_b td_loss_b / B; dq = w_b/B * dl/dq.
+ * actor: c = clip(dqda, +-dqda_clipping) when clip, dqda at row stride ld_dqda;
+ *   loss = sum_b w_b sum_{t,k} c^2 / (B*A); dy [B*(T-1), A] = (amax-amin)/2 * (-2 w_b c / (B*A)).
+ * partials: >= B200RL_DDPG_SEQ_MAX_BLOCKS floats of scratch; ticket: a uint32 that is 0 before the
+ * launch and is left at 0.  Fixed-order sums: repeated calls return the same bits, and with
+ * T = 2 dq and dy equal the feed-forward kernels' bits.  nan_flag may be NULL. */
+#define B200RL_DDPG_SEQ_MAX_BLOCKS 1024
+int b200rl_ddpg_seq_critic_loss(const float* q, const float* tq, const float* reward,
+                                const float* discount, int64_t ld, int64_t stride,
+                                const float* weights, int64_t weight_stride, int64_t B, int64_t T,
+                                float gamma, float reward_scale, int loss_kind, float* loss,
+                                float* dq, int32_t* nan_flag, float* partials, uint32_t* ticket,
+                                void* stream);
+int b200rl_ddpg_seq_actor_loss(const float* dqda, int64_t ld_dqda, const float* weights,
+                               int64_t weight_stride, int64_t B, int64_t T, int64_t A, int clip,
+                               float dqda_clipping, const float* amin, const float* amax,
+                               float* loss, float* dy, int32_t* nan_flag, float* partials,
+                               uint32_t* ticket, void* stream);
 /* One Ornstein-Uhlenbeck step: state [A] <- (1-damping)*state + stddev*z, z = noise_in [A] or
  * N(0,1) by Philox + Box-Muller on element k of rng_call_dev uint64[2] {call, ticket} (the call
  * advances only when the device draws; the ticket slot is used either way); then
