@@ -16,6 +16,7 @@ ACT_NONE, ACT_RELU, ACT_TANH = 0, 1, 2
 LOSS_HUBER, LOSS_SQUARED = 0, 1
 DQN_SEQ_MAX_BLOCKS = 1024   # B200RL_DQN_SEQ_MAX_BLOCKS: partials of b200rl_dqn_seq_td_loss
 DDPG_SEQ_MAX_BLOCKS = 1024  # B200RL_DDPG_SEQ_MAX_BLOCKS: partials of b200rl_ddpg_seq_*_loss
+SAC_SEQ_MAX_BLOCKS = 1024   # B200RL_SAC_SEQ_MAX_BLOCKS: partials of b200rl_sac_seq_*_loss
 
 c_void_p = ctypes.c_void_p
 c_i64 = ctypes.c_int64
@@ -108,6 +109,12 @@ SIGNATURES = {
     'b200rl_sac_actor_loss': [_P, _P, _P, _P, _P, c_i64, c_f32, c_f32, _P, _P, _P, _P, _P, _P],
     'b200rl_sac_alpha_loss': [_P, _P, _P, c_i64, c_f32, c_int, c_f32, c_f32, _P, _P, _P, _P],
     'b200rl_concat2': [_P, c_i64, c_i64, _P, c_i64, c_i64, c_i64, _P, _P],
+    'b200rl_sac_seq_critic_loss': [_P, _P, _P, _P, _P, _P, _P, c_i64, c_i64, _P, c_i64, _P, c_i64,
+                                   c_i64, c_f32, c_f32, c_f32, _P, _P, _P, _P, _P, _P, _P],
+    'b200rl_sac_seq_actor_loss': [_P, _P, _P, _P, c_i64, _P, c_i64, c_i64, c_f32, _P, _P, _P, _P,
+                                  _P, _P, _P, _P],
+    'b200rl_sac_seq_alpha_loss': [_P, _P, c_i64, _P, c_i64, c_i64, c_f32, c_int, c_f32, _P, _P, _P,
+                                  _P, _P, _P],
     'b200rl_td3_scale_to_spec': [_P, c_i64, c_i64, c_i64, _P, _P, c_f32, c_f32, _P, c_u64, _P, c_int,
                                  _P, c_i64, _P],
     'b200rl_td3_critic_loss': [_P, _P, _P, _P, _P, _P, _P, c_i64, c_f32, c_f32, c_int, _P, _P, _P,

@@ -75,6 +75,11 @@ class CqlSacAgent(sac_agent.SacAgent):
                log_cql_alpha_clipping=None, softmax_temperature=1.0, bc_debug_mode=False,
                debug_summaries=False, summarize_grads_and_vars=False, train_step_counter=None,
                name=None):
+    for net in (critic_network, actor_network, critic_network_2, target_critic_network,
+                target_critic_network_2):
+      if net is not None and getattr(net, 'state_spec', ()):
+        raise NotImplementedError('CqlSacAgent supports feed-forward networks only: recurrent '
+                                  'CQL-SAC is not implemented.')
     if int(num_cql_samples) < 1:
       raise ValueError('num_cql_samples must be >= 1.')
     if float(softmax_temperature) <= 0:

@@ -32,6 +32,7 @@ from agents_b200 import _lib
 from agents_b200.agents import tf_agent
 from agents_b200.agents.ppo import ppo_policy
 from agents_b200.networks import network as network_lib
+from agents_b200.policies import actor_policy
 from agents_b200.specs import tensor_spec
 from agents_b200.trajectories import trajectory
 from agents_b200.utils import nest
@@ -61,6 +62,7 @@ class PPOAgent(tf_agent.TFAgent):
                name=None, seed=0):
     if actor_net is None or value_net is None:
       raise ValueError('actor_net and value_net must be given.')
+    actor_policy.reject_tanh_normal(actor_net, 'PPOAgent')
     if not use_gae:
       raise NotImplementedError('Only use_gae=True is supported (PPO examples use GAE).')
     if shared_vars_l2_reg:

@@ -33,6 +33,7 @@ class PPOPolicy(actor_policy.ActorPolicy):
   def __init__(self, time_step_spec, action_spec, actor_net, value_net,
                observation_normalizer=None, clip=True, collect=True,
                compute_value_and_advantage_in_train=True, seed=0):
+    actor_policy.reject_tanh_normal(actor_net, 'PPOPolicy')
     info_spec = ()
     if collect:
       info_spec = {'dist_params': actor_net.dist_params_spec()}

@@ -16,6 +16,26 @@ sample, fused alpha loss, Adam; fused Polyak over both critics.
 
 Extension (keyword-only): `train(..., noise=(eps_next, eps_actor, eps_alpha))` supplies the
 three N(0,1) draws ("oracle mode") so parity tests are independent of the RNG stream.
+
+Recurrent SAC: with a tanh-Normal ActorDistributionRnnNetwork actor
+(continuous_projection_net=TanhNormalProjectionNetwork) and CriticRnnNetwork critics the agent
+trains on whole [B, T] sequences, T >= 2 (train_sequence_length None;
+data_converter.AsTransition(squeeze_time_dim=False)).  Transition t < T-1 of sequence b is row
+b*(T-1) + t.  Every network runs from the zero state with a reset at FIRST: the actor's a' and the
+target critics over observation[:, 1:] with next_step_type[:, :-1]; the online critics and the
+actor's actor-step and alpha-step samples over observation[:, :-1] with step_type[:, :-1].
+  * Each loss sums over time, then applies the weights, then takes the mean over B; there is no
+    LAST mask, as in the reference.
+  * The actor loss's dQ/da comes through each critic's full BPTT (a_t moves every later Q), with
+    input gradients only: the critics' own gradients are not touched.
+  * The noise draws of `train(..., noise=...)` are [B, T-1, A].
+Device work per recurrent step (csrc/sac.cu, lstm.cu, nn.cu, optim.cu): actor sequence forward +
+sample over observation[:, 1:], 2 target-critic sequence forwards, 2 critic sequence forwards,
+b200rl_sac_seq_critic_loss (reward and discount read in place from the [B, T] experience), 2
+critic BPTT backwards, Adam; actor sequence forward + sample, 2 critic sequence forwards,
+b200rl_sac_seq_actor_loss, 2 input-gradient-only critic BPTTs, sample backward, actor BPTT, Adam;
+actor sequence forward + sample, b200rl_sac_seq_alpha_loss, Adam; one Polyak launch.
+Data-parallel recurrent training raises.
 """
 import collections
 
@@ -23,6 +43,9 @@ import torch
 
 from agents_b200 import _lib
 from agents_b200.agents import tf_agent
+from agents_b200.agents.ddpg import ddpg_agent
+from agents_b200.networks import actor_distribution_rnn_network
+from agents_b200.networks import critic_rnn_network
 from agents_b200.networks import network as network_lib
 from agents_b200.policies import tf_policy
 from agents_b200.trajectories import policy_step
@@ -36,12 +59,33 @@ _Batch = collections.namedtuple('_Batch', ('obs', 'obs2', 'action', 'reward', 'd
 _SAC_SEED_TAG = 0x5341435F53414D50
 
 
+def _check_recurrent(actor_network, critics):
+  """True for a tanh-Normal ActorDistributionRnnNetwork actor with CriticRnnNetwork critics, False
+  for feed-forward networks only; any other stateful combination raises NotImplementedError."""
+  nets = [actor_network] + [c for c in critics if c is not None]
+  if not any(getattr(n, 'state_spec', ()) for n in nets):
+    return False
+  if not (isinstance(actor_network, actor_distribution_rnn_network.ActorDistributionRnnNetwork)
+          and actor_network.tanh_normal and
+          all(isinstance(c, critic_rnn_network.CriticRnnNetwork) for c in nets[1:])):
+    raise NotImplementedError(
+        'SacAgent supports feed-forward networks, or a recurrent ActorDistributionRnnNetwork '
+        'actor with continuous_projection_net=TanhNormalProjectionNetwork and CriticRnnNetwork '
+        'critics; got {}.'.format(', '.join(type(n).__name__ for n in nets)))
+  return True
+
+
 class SacPolicy(tf_policy.TFPolicy):
-  """ActorPolicy over the tanh-Normal actor: sampled (collect) or mode (greedy) actions."""
+  """ActorPolicy over the tanh-Normal actor: sampled (collect) or mode (greedy) actions.
+
+  A recurrent actor (ActorDistributionRnnNetwork with the tanh-Normal head) makes the policy
+  stateful: `policy_state_spec` is the actor's `state_spec`, and each call runs one [B, 1] step
+  from the given state (the zero state where step_type is FIRST) and returns the new state."""
 
   def __init__(self, time_step_spec, action_spec, actor_network, training=False, seed=0,
                greedy=False):
-    super().__init__(time_step_spec, action_spec)
+    super().__init__(time_step_spec, action_spec,
+                     policy_state_spec=getattr(actor_network, 'state_spec', ()))
     self._actor = actor_network
     self._greedy = greedy
     self._seed = (int(seed) ^ _SAC_SEED_TAG) & 0xFFFFFFFFFFFFFFFF
@@ -50,13 +94,31 @@ class SacPolicy(tf_policy.TFPolicy):
   def variables(self):
     return self._actor.variables
 
-  def sample(self, observation, noise=None, keep=False):
-    """Returns (action [N, A], logp [N], ctx) with ctx = (head, tape, u, eps) when keep."""
-    a_dim = self._actor.num_actions
-    if keep:
+  def get_initial_state(self, batch_size=None):
+    if not self._policy_state_spec:
+      return ()
+    return self._actor.get_initial_state(batch_size)
+
+  def sample(self, observation, noise=None, keep=False, step_type=None):
+    """Returns (action [N, A], logp [N], ctx) with ctx = (head, tape, u, eps) when keep.  A
+    recurrent actor takes observation [B, T, ...] with step_type [B, T] and runs from the zero
+    state; N = B*T in batch-major order."""
+    if self._policy_state_spec:
+      if keep:
+        head, tape = self._actor.forward_train(observation, step_type)
+      else:
+        (head, _), tape = self._actor.distribution_params(observation, step_type), None
+    elif keep:
       head, tape = self._actor.forward_train(observation)
     else:
       (head, _), tape = self._actor(observation), None
+    action, logp, u, eps = self._draw(head, noise, keep)
+    return action, logp, (head, tape, u, eps)
+
+  def _draw(self, head, noise, keep):
+    """(action, logp, u, eps) from the [N, 2A] head; u and eps (kept for the backward) are None
+    unless keep."""
+    a_dim = self._actor.num_actions
     n = head.shape[0]
     dev = head.device
     if self._rng is None or self._rng.device != dev:
@@ -70,7 +132,7 @@ class SacPolicy(tf_policy.TFPolicy):
     _lib.call('b200rl_sac_sample', _lib.ptr(head), n, a_dim, _lib.ptr(self._actor.action_min),
               _lib.ptr(self._actor.action_max), _lib.ptr(noise), self._seed, _lib.ptr(self._rng),
               _lib.ptr(action), a_dim, _lib.ptr(logp), _lib.ptr(u), _lib.ptr(eps), _lib.stream())
-    return action, logp, (head, tape, u, eps)
+    return action, logp, u, eps
 
   def _action(self, time_step, policy_state, seed):
     noise = None
@@ -78,8 +140,16 @@ class SacPolicy(tf_policy.TFPolicy):
       n = time_step.step_type.shape[0]
       noise = torch.zeros((n, self._actor.num_actions), dtype=torch.float32,
                           device=time_step.step_type.device)
-    action, _, _ = self.sample(time_step.observation, noise=noise)
-    return policy_step.PolicyStep(action, policy_state, ())
+    if not self._policy_state_spec:
+      action, _, _ = self.sample(time_step.observation, noise=noise)
+      return policy_step.PolicyStep(action, policy_state, ())
+    if len(nest.flatten(policy_state)) != len(nest.flatten(self._policy_state_spec)):
+      raise ValueError('This SacPolicy is stateful (its actor is recurrent): pass the policy_state '
+                       'from get_initial_state(batch_size) or from the previous action().')
+    head, state = self._actor.distribution_params(time_step.observation, time_step.step_type,
+                                                  policy_state)
+    action, _, _, _ = self._draw(head, noise, keep=False)
+    return policy_step.PolicyStep(action, state, ())
 
 
 class SacAgent(tf_agent.TFAgent):
@@ -93,11 +163,8 @@ class SacAgent(tf_agent.TFAgent):
                initial_log_alpha=0.0, use_log_alpha_in_alpha_loss=True, target_entropy=None,
                gradient_clipping=None, debug_summaries=False, summarize_grads_and_vars=False,
                train_step_counter=None, name=None, seed=0):
-    for net in (critic_network, actor_network, critic_network_2, target_critic_network,
-                target_critic_network_2):
-      if net is not None and getattr(net, 'state_spec', ()):
-        raise NotImplementedError('SacAgent supports feed-forward networks only: a recurrent '
-                                  'network needs sequence training.')
+    self._recurrent = _check_recurrent(actor_network, (
+        critic_network, critic_network_2, target_critic_network, target_critic_network_2))
     flat_action_spec = nest.flatten(action_spec)
     if len(flat_action_spec) != 1:
       raise NotImplementedError('Only a single continuous action tensor is supported.')
@@ -150,12 +217,15 @@ class SacAgent(tf_agent.TFAgent):
     self._train_policy = SacPolicy(time_step_spec, action_spec, actor_network, seed=seed + 1)
     super(SacAgent, self).__init__(
         time_step_spec, action_spec, policy=policy, collect_policy=collect_policy,
-        train_sequence_length=2, debug_summaries=debug_summaries,
+        train_sequence_length=None if self._recurrent else 2, debug_summaries=debug_summaries,
         summarize_grads_and_vars=summarize_grads_and_vars, train_step_counter=train_step_counter,
         device=device)
     self._nan_flag = torch.zeros(1, dtype=torch.int32, device=device)
     self.replicas = 1
     self._grad_sync = None
+    if self._recurrent:   # b200rl_sac_seq_*_loss scratch: block partials and a last-block ticket
+      self._seq_partials = torch.empty(_lib.SAC_SEQ_MAX_BLOCKS, dtype=torch.float32, device=device)
+      self._seq_ticket = torch.zeros(1, dtype=torch.int32, device=device)
 
   @property
   def log_alpha(self):
@@ -166,13 +236,21 @@ class SacAgent(tf_agent.TFAgent):
     common.soft_variables_update(self._critic_params, self._target_params, tau=1.0)
 
   def _train(self, experience, weights=None, noise=None):
-    b = self._batch(experience, weights)
     n_next = n_actor = n_alpha = None
     if noise is not None:
       n_next, n_actor, n_alpha = noise
-    closs = self._critic_step(b, n_next)
-    aloss = self._actor_step(b, n_actor)
-    alloss = self._alpha_step(b, n_alpha)
+    if self._recurrent:
+      if self.replicas != 1 or self._grad_sync is not None:
+        raise NotImplementedError('Recurrent SacAgent does not support data-parallel training.')
+      b = self._seq_batch(experience, weights)
+      closs = self._seq_critic_step(b, n_next)
+      aloss = self._seq_actor_step(b, n_actor)
+      alloss = self._seq_alpha_step(b, n_alpha)
+    else:
+      b = self._batch(experience, weights)
+      closs = self._critic_step(b, n_next)
+      aloss = self._actor_step(b, n_actor)
+      alloss = self._alpha_step(b, n_alpha)
     self._bump_train_step(1)
     self._update_target()
     total = closs + aloss + alloss
@@ -276,6 +354,70 @@ class SacAgent(tf_agent.TFAgent):
               _lib.stream())
     if self._grad_sync is not None:
       self._grad_sync(self._dlog_alpha)
+    self._alpha_optimizer.apply_flat(self._log_alpha, self._dlog_alpha)
+    return alloss
+
+  # ---- recurrent SAC -----------------------------------------------------------------------
+  # DDPG's unpacking of the [B, T] experience into the [B, T-1] windows of the transitions
+  _seq_batch = ddpg_agent.DdpgAgent._seq_batch
+
+  def _seq_scratch(self):
+    return _lib.ptr(self._nan_flag), _lib.ptr(self._seq_partials), _lib.ptr(self._seq_ticket)
+
+  def _seq_critic_step(self, b, noise):
+    """The [B, T-1] critic loss against the target critics over observation[:, 1:]; both critics'
+    BPTT gradients, one optimiser step."""
+    c1, c2 = self._critic_network_1, self._critic_network_2
+    a2, logp2, _ = self._train_policy.sample(b.obs2, noise=noise, step_type=b.step_type2)
+    tq1, _ = self._target_critic_network_1((b.obs2, a2), b.step_type2)
+    tq2, _ = self._target_critic_network_2((b.obs2, a2), b.step_type2)
+    q1, tape1 = c1.forward_train((b.obs, b.action), b.step_type)
+    q2, tape2 = c2.forward_train((b.obs, b.action), b.step_type)
+    n = b.B * (b.T - 1)
+    closs, dq1, dq2 = self._new(1), self._new(n), self._new(n)
+    _lib.call('b200rl_sac_seq_critic_loss', _lib.ptr(q1), _lib.ptr(q2), _lib.ptr(tq1),
+              _lib.ptr(tq2), _lib.ptr(logp2), _lib.dptr(b.reward), _lib.dptr(b.discount),
+              b.reward.stride(0), b.reward.stride(1), _lib.ptr(b.weights), b.w_stride,
+              _lib.ptr(self._log_alpha), b.B, b.T, float(self._gamma),
+              float(self._reward_scale_factor), float(self._critic_loss_weight), _lib.ptr(closs),
+              _lib.ptr(dq1), _lib.ptr(dq2), *self._seq_scratch(), _lib.stream())
+    self._apply_critic_grads(tape1, dq1, tape2, dq2)
+    return closs
+
+  def _seq_actor_step(self, b, noise):
+    """The [B, T-1] actor loss against the updated critics: dQ/da of each critic through its
+    BPTT (input gradients only), the sample backward, the actor BPTT, one optimiser step."""
+    c1, c2, actor = self._critic_network_1, self._critic_network_2, self._actor_network
+    n, st = b.B * (b.T - 1), _lib.stream()
+    a, logp, (head, atape, u, eps) = self._train_policy.sample(b.obs, noise=noise, keep=True,
+                                                                step_type=b.step_type)
+    qa1, t1 = c1.forward_train((b.obs, a), b.step_type)
+    qa2, t2 = c2.forward_train((b.obs, a), b.step_type)
+    aloss, dlogp, dqa1, dqa2 = self._new(1), self._new(n), self._new(n), self._new(n)
+    _lib.call('b200rl_sac_seq_actor_loss', _lib.ptr(qa1), _lib.ptr(qa2), _lib.ptr(logp),
+              _lib.ptr(b.weights), b.w_stride, _lib.ptr(self._log_alpha), b.B, b.T,
+              float(self._actor_loss_weight), _lib.ptr(aloss), _lib.ptr(dlogp), _lib.ptr(dqa1),
+              _lib.ptr(dqa2), *self._seq_scratch(), st)
+    da1, da2 = c1.action_gradient(t1, dqa1), c2.action_gradient(t2, dqa2)
+    if da1.stride() != da2.stride() or da1.stride(1) != 1:   # sample_bwd takes one row stride
+      da1, da2 = da1.contiguous(), da2.contiguous()
+    dhead = self._new(n, 2 * actor.num_actions)
+    _lib.call('b200rl_sac_sample_bwd', _lib.ptr(head), _lib.ptr(u), _lib.ptr(eps),
+              _lib.ptr(actor.action_min), _lib.ptr(actor.action_max), _lib.dptr(da1),
+              _lib.dptr(da2), da1.stride(0), _lib.ptr(dlogp), n, actor.num_actions,
+              _lib.ptr(dhead), st)
+    agrads = actor.backward(atape, dhead)
+    self._actor_optimizer.apply_flat(actor.flat_params, agrads)
+    return aloss
+
+  def _seq_alpha_step(self, b, noise):
+    """The [B, T-1] alpha loss against the updated actor, one optimiser step."""
+    _, logp3, _ = self._train_policy.sample(b.obs, noise=noise, step_type=b.step_type)
+    alloss = self._new(1)
+    _lib.call('b200rl_sac_seq_alpha_loss', _lib.ptr(logp3), _lib.ptr(b.weights), b.w_stride,
+              _lib.ptr(self._log_alpha), b.B, b.T, float(self._target_entropy),
+              int(self._use_log_alpha_in_alpha_loss), float(self._alpha_loss_weight),
+              _lib.ptr(alloss), _lib.ptr(self._dlog_alpha), *self._seq_scratch(), _lib.stream())
     self._alpha_optimizer.apply_flat(self._log_alpha, self._dlog_alpha)
     return alloss
 

@@ -284,4 +284,22 @@ __device__ __forceinline__ float block_sum(float v, float* smem32) {
   return r;
 }
 
+// ---- multi-CTA sequence-loss totals (ddpg.cu, sac.cu) -------------------------------------------
+// Every block stores its block_sum of `partial` in partials[blockIdx.x]; the block that takes the
+// last ticket adds the partials in index order and returns the total there (threads of other
+// blocks return 0 and must not use it).  No float atomics: the sum has a fixed order per grid.
+__device__ __forceinline__ float seq_loss_total(float partial, float* partials, uint32_t* ticket,
+                                                float* red, bool* last) {
+  const float total = block_sum(partial, red);
+  if (threadIdx.x == 0) {
+    partials[blockIdx.x] = total;
+    *last = last_block_ticket(ticket);
+  }
+  __syncthreads();
+  if (!*last) return 0.f;
+  float s = 0.f;
+  for (unsigned i = threadIdx.x; i < gridDim.x; i += blockDim.x) s += __ldcg(partials + i);
+  return block_sum(s, red);
+}
+
 }  // namespace b200rl

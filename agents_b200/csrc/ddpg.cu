@@ -121,22 +121,6 @@ __global__ void ou_noise_kernel(const float* __restrict__ loc, int64_t ld_loc, i
 // partials in index order.  Every sum has a fixed order for a given shape, so repeated launches and
 // graph replays give the same bits.  With T-1 = 1, dq and dy are the feed-forward kernels' bits.
 
-// Adds the block partials in index order in the block that takes the last ticket; returns the
-// total there (threads of other blocks return 0 and must not use it).
-__device__ __forceinline__ float ddpg_seq_total(float partial, float* partials, uint32_t* ticket,
-                                                float* red, bool* last) {
-  const float total = block_sum(partial, red);
-  if (threadIdx.x == 0) {
-    partials[blockIdx.x] = total;
-    *last = last_block_ticket(ticket);
-  }
-  __syncthreads();
-  if (!*last) return 0.f;
-  float s = 0.f;
-  for (unsigned i = threadIdx.x; i < gridDim.x; i += blockDim.x) s += __ldcg(partials + i);
-  return block_sum(s, red);
-}
-
 // y = reward_scale r[b, t] + gamma d[b, t] tq[r];  td_loss_b = sum_t l(y - q[r]);
 // loss = sum_b w_b td_loss_b / B;  dq[r] = w_b / B * dl/dq.  No LAST mask (ddpg_agent.py's TODO).
 template <int G>
@@ -168,7 +152,7 @@ __global__ void __launch_bounds__(256) ddpg_seq_critic_loss_kernel(
     const float row = grp_sum<G>((float)s);
     if (live && lane == 0) partial += row * w;
   }
-  const float total = ddpg_seq_total(partial, partials, ticket, red, &last);
+  const float total = seq_loss_total(partial, partials, ticket, red, &last);
   if (last && threadIdx.x == 0) {
     const float out = total / (float)B;
     loss[0] = out;
@@ -206,7 +190,7 @@ __global__ void __launch_bounds__(256) ddpg_seq_actor_loss_kernel(
     const float row = grp_sum<G>((float)s);
     if (live && lane == 0) partial += row;
   }
-  const float total = ddpg_seq_total(partial, partials, ticket, red, &last);
+  const float total = seq_loss_total(partial, partials, ticket, red, &last);
   if (last && threadIdx.x == 0) {
     const float out = total * inv_n;
     loss[0] = out;

@@ -164,7 +164,164 @@ __global__ void concat2_kernel(const float* __restrict__ a, int64_t lda, int64_t
   out[i] = k < da ? a[n * lda + k] : b[n * ldb + (k - da)];
 }
 
+// ---- recurrent SAC: the three losses over the [B, T-1] transitions of a sequence ---------------
+// Row r = b*(T-1) + t of q1 / q2 / tq1 / tq2 / logp and of the gradients is transition t of
+// sequence b.  G lanes per batch row take its steps l, l + G, ... in order and accumulate in
+// double; the G lane sums meet in a fixed shuffle tree, the row sum is weighted once, and
+// seq_loss_total adds the block partials in index order.  Every sum has a fixed order for a given
+// shape, so repeated launches and graph replays give the same bits.  With T-1 = 1 the per-row
+// gradients are the feed-forward kernels' bits.  A row of weight 0 adds exactly 0.
+
+// tq = min(tq1, tq2) - alpha next_logp;  y = reward_scale r[b, t] + gamma d[b, t] tq;
+// loss = loss_weight sum_b w_b sum_t [(y - q1)^2 + (y - q2)^2] / B;  dq_i = -2 (y - q_i) c with
+// c = loss_weight w_b / B.  No LAST mask (as sac_agent.py with AsTransition).
+template <int G>
+__global__ void __launch_bounds__(256) sac_seq_critic_loss_kernel(
+    const float* __restrict__ q1, const float* __restrict__ q2, const float* __restrict__ tq1,
+    const float* __restrict__ tq2, const float* __restrict__ next_logp,
+    const float* __restrict__ reward, const float* __restrict__ discount, int64_t ld, int64_t st,
+    const float* __restrict__ weights, int64_t w_stride, const float* __restrict__ log_alpha,
+    int64_t B, int64_t Tm, float gamma, float reward_scale, float loss_weight,
+    float* __restrict__ loss, float* __restrict__ dq1, float* __restrict__ dq2, int32_t* nan_flag,
+    float* partials, uint32_t* ticket) {
+  pdl_prologue();
+  __shared__ float red[32];
+  __shared__ bool last;
+  const float alpha = expf(log_alpha[0]);
+  const float global_batch = (float)B;
+  float partial = 0.f;
+  B200RL_GROUP_ROWS(G, B) {
+    const bool live = n < B;
+    const int64_t b = live ? n : n0;
+    const float w = weights ? weights[b * w_stride] : 1.f;
+    const float c = loss_weight * w / global_batch;
+    double s = 0.0;   // a lane may sum ~1000 steps: accumulate in double, round once
+    for (int64_t t = lane; t < Tm; t += G) {
+      const int64_t r = b * Tm + t;
+      const float tq = fminf(tq1[r], tq2[r]) - alpha * next_logp[r];
+      const float y = reward_scale * reward[b * ld + t * st] + gamma * discount[b * ld + t * st] *
+                                                                   tq;
+      const float e1 = y - q1[r], e2 = y - q2[r];
+      s += e1 * e1 + e2 * e2;
+      if (live) {
+        dq1[r] = -2.f * e1 * c;
+        dq2[r] = -2.f * e2 * c;
+      }
+    }
+    const float row = grp_sum<G>((float)s);
+    if (live && lane == 0) partial += (weights && w == 0.f) ? 0.f : row * w;
+  }
+  const float total = seq_loss_total(partial, partials, ticket, red, &last);
+  if (last && threadIdx.x == 0) {
+    const float out = loss_weight * total / global_batch;
+    loss[0] = out;
+    if (nan_flag && !isfinite(out)) *nan_flag = 1;
+  }
+}
+
+// loss = loss_weight sum_b w_b sum_t (alpha logp - min(q1, q2)) / B;  with k = loss_weight w_b / B:
+// dlogp = alpha k, and -k to q1 where q1 <= q2 (tf.minimum's gradient routing), else to q2.
+template <int G>
+__global__ void __launch_bounds__(256) sac_seq_actor_loss_kernel(
+    const float* __restrict__ q1, const float* __restrict__ q2, const float* __restrict__ logp,
+    const float* __restrict__ weights, int64_t w_stride, const float* __restrict__ log_alpha,
+    int64_t B, int64_t Tm, float loss_weight, float* __restrict__ loss,
+    float* __restrict__ dlogp, float* __restrict__ dq1, float* __restrict__ dq2,
+    int32_t* nan_flag, float* partials, uint32_t* ticket) {
+  pdl_prologue();
+  __shared__ float red[32];
+  __shared__ bool last;
+  const float alpha = expf(log_alpha[0]);
+  const float global_batch = (float)B;
+  float partial = 0.f;
+  B200RL_GROUP_ROWS(G, B) {
+    const bool live = n < B;
+    const int64_t b = live ? n : n0;
+    const float w = weights ? weights[b * w_stride] : 1.f;
+    const float k = loss_weight * w / global_batch;
+    double s = 0.0;
+    for (int64_t t = lane; t < Tm; t += G) {
+      const int64_t r = b * Tm + t;
+      const float a = q1[r], c = q2[r];
+      s += alpha * logp[r] - fminf(a, c);
+      if (live) {
+        const bool first = a <= c;
+        dlogp[r] = alpha * k;
+        dq1[r] = first ? -k : 0.f;
+        dq2[r] = first ? 0.f : -k;
+      }
+    }
+    const float row = grp_sum<G>((float)s);
+    if (live && lane == 0) partial += (weights && w == 0.f) ? 0.f : row * w;
+  }
+  const float total = seq_loss_total(partial, partials, ticket, red, &last);
+  if (last && threadIdx.x == 0) {
+    const float out = loss_weight * total / global_batch;
+    loss[0] = out;
+    if (nan_flag && !isfinite(out)) *nan_flag = 1;
+  }
+}
+
+// S = sum_b w_b sum_t (-logp - target_entropy);  loss = loss_weight coef S / B and
+// dlog_alpha = loss_weight dcoef S / B, coef = log_alpha (dcoef 1) or alpha (dcoef alpha).
+template <int G>
+__global__ void __launch_bounds__(256) sac_seq_alpha_loss_kernel(
+    const float* __restrict__ logp, const float* __restrict__ weights, int64_t w_stride,
+    const float* __restrict__ log_alpha, int64_t B, int64_t Tm, float target_entropy,
+    int use_log_alpha, float loss_weight, float* __restrict__ loss,
+    float* __restrict__ dlog_alpha, int32_t* nan_flag, float* partials, uint32_t* ticket) {
+  pdl_prologue();
+  __shared__ float red[32];
+  __shared__ bool last;
+  float partial = 0.f;
+  B200RL_GROUP_ROWS(G, B) {
+    const bool live = n < B;
+    const int64_t b = live ? n : n0;
+    const float w = weights ? weights[b * w_stride] : 1.f;
+    double s = 0.0;
+    for (int64_t t = lane; t < Tm; t += G) s += -logp[b * Tm + t] - target_entropy;
+    const float row = grp_sum<G>((float)s);
+    if (live && lane == 0) partial += (weights && w == 0.f) ? 0.f : row * w;
+  }
+  const float total = seq_loss_total(partial, partials, ticket, red, &last);
+  if (last && threadIdx.x == 0) {
+    const float la = log_alpha[0];
+    const float coef = use_log_alpha ? la : expf(la);
+    const float dcoef = use_log_alpha ? 1.f : expf(la);
+    const float out = loss_weight * coef * total / (float)B;
+    loss[0] = out;
+    dlog_alpha[0] = loss_weight * dcoef * total / (float)B;
+    if (nan_flag && !isfinite(out)) *nan_flag = 1;
+  }
+}
+
 }  // namespace b200rl
+
+namespace {
+
+// Lanes per row, grid and argument checks shared by the three sequence-loss entry points.
+int sac_seq_shape(const char* name, int64_t B, int64_t T, int64_t weight_stride, int* G,
+                  unsigned* blocks) {
+  B200RL_CHECK_ARG(B >= 1, "%s: B=%lld", name, (long long)B);
+  B200RL_CHECK_ARG(T >= 2, "Trajectory frame count must be at least 2, but saw %lld", (long long)T);
+  B200RL_CHECK_ARG(weight_stride >= 0, "%s: weight_stride must be >= 0", name);
+  *G = b200rl::lane_group(T - 1);
+  *blocks = b200rl::group_blocks(B, *G, B200RL_SAC_SEQ_MAX_BLOCKS);
+  return B200RL_OK;
+}
+
+}  // namespace
+
+// G is one of 1, 8, 32 (lane_group); the launch picks the matching instantiation.
+#define B200RL_SAC_SEQ_LAUNCH(kernel, G, blocks, st, ...)         \
+  do {                                                            \
+    if ((G) == 1)                                                 \
+      B200RL_LAUNCH(kernel<1>, blocks, 256, 0, st, __VA_ARGS__);  \
+    else if ((G) == 8)                                            \
+      B200RL_LAUNCH(kernel<8>, blocks, 256, 0, st, __VA_ARGS__);  \
+    else                                                          \
+      B200RL_LAUNCH(kernel<32>, blocks, 256, 0, st, __VA_ARGS__); \
+  } while (0)
 
 using namespace b200rl;
 
@@ -237,6 +394,67 @@ int b200rl_concat2(const float* a, int64_t lda, int64_t da, const float* b, int6
                    "concat2: bad argument");
   B200RL_LAUNCH(concat2_kernel, blocks_of_256(N * (da + db)), 256, 0, (cudaStream_t)stream, a, lda, da, b, ldb, db, N, out);
   B200RL_CHECK_LAUNCH("concat2");
+  return B200RL_OK;
+}
+
+int b200rl_sac_seq_critic_loss(const float* q1, const float* q2, const float* tq1,
+                               const float* tq2, const float* next_logp, const float* reward,
+                               const float* discount, int64_t ld, int64_t stride,
+                               const float* weights, int64_t weight_stride,
+                               const float* log_alpha_dev, int64_t B, int64_t T, float gamma,
+                               float reward_scale, float loss_weight, float* loss, float* dq1,
+                               float* dq2, int32_t* nan_flag, float* partials, uint32_t* ticket,
+                               void* stream) {
+  B200RL_CHECK_ARG(q1 && q2 && tq1 && tq2 && next_logp && reward && discount && log_alpha_dev &&
+                       loss && dq1 && dq2 && partials && ticket,
+                   "sac_seq_critic_loss: NULL argument");
+  B200RL_CHECK_ARG(ld >= 0 && stride >= 0, "sac_seq_critic_loss: strides must be >= 0");
+  int G;
+  unsigned blocks;
+  const int rc = sac_seq_shape("sac_seq_critic_loss", B, T, weight_stride, &G, &blocks);
+  if (rc != B200RL_OK) return rc;
+  B200RL_SAC_SEQ_LAUNCH(sac_seq_critic_loss_kernel, G, blocks, (cudaStream_t)stream, q1, q2, tq1,
+                        tq2, next_logp, reward, discount, ld, stride, weights, weight_stride,
+                        log_alpha_dev, B, T - 1, gamma, reward_scale, loss_weight, loss, dq1, dq2,
+                        nan_flag, partials, ticket);
+  B200RL_CHECK_LAUNCH("sac_seq_critic_loss");
+  return B200RL_OK;
+}
+
+int b200rl_sac_seq_actor_loss(const float* q1, const float* q2, const float* logp,
+                              const float* weights, int64_t weight_stride,
+                              const float* log_alpha_dev, int64_t B, int64_t T, float loss_weight,
+                              float* loss, float* dlogp, float* dq1, float* dq2, int32_t* nan_flag,
+                              float* partials, uint32_t* ticket, void* stream) {
+  B200RL_CHECK_ARG(q1 && q2 && logp && log_alpha_dev && loss && dlogp && dq1 && dq2 && partials &&
+                       ticket,
+                   "sac_seq_actor_loss: NULL argument");
+  int G;
+  unsigned blocks;
+  const int rc = sac_seq_shape("sac_seq_actor_loss", B, T, weight_stride, &G, &blocks);
+  if (rc != B200RL_OK) return rc;
+  B200RL_SAC_SEQ_LAUNCH(sac_seq_actor_loss_kernel, G, blocks, (cudaStream_t)stream, q1, q2, logp,
+                        weights, weight_stride, log_alpha_dev, B, T - 1, loss_weight, loss, dlogp,
+                        dq1, dq2, nan_flag, partials, ticket);
+  B200RL_CHECK_LAUNCH("sac_seq_actor_loss");
+  return B200RL_OK;
+}
+
+int b200rl_sac_seq_alpha_loss(const float* logp, const float* weights, int64_t weight_stride,
+                              const float* log_alpha_dev, int64_t B, int64_t T,
+                              float target_entropy, int use_log_alpha, float loss_weight,
+                              float* loss, float* dlog_alpha, int32_t* nan_flag, float* partials,
+                              uint32_t* ticket, void* stream) {
+  B200RL_CHECK_ARG(logp && log_alpha_dev && loss && dlog_alpha && partials && ticket,
+                   "sac_seq_alpha_loss: NULL argument");
+  int G;
+  unsigned blocks;
+  const int rc = sac_seq_shape("sac_seq_alpha_loss", B, T, weight_stride, &G, &blocks);
+  if (rc != B200RL_OK) return rc;
+  B200RL_SAC_SEQ_LAUNCH(sac_seq_alpha_loss_kernel, G, blocks, (cudaStream_t)stream, logp, weights,
+                        weight_stride, log_alpha_dev, B, T - 1, target_entropy, use_log_alpha,
+                        loss_weight, loss, dlog_alpha, nan_flag, partials, ticket);
+  B200RL_CHECK_LAUNCH("sac_seq_alpha_loss");
   return B200RL_OK;
 }
 

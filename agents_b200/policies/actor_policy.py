@@ -24,6 +24,13 @@ from agents_b200.utils import nest
 _ACTOR_SEED_TAG = 0x4143544F52504F4C
 
 
+def reject_tanh_normal(actor_network, who):
+  """The tanh-Normal recurrent actor emits a raw [N, 2A] head that only SacPolicy samples."""
+  if getattr(actor_network, 'tanh_normal', False):
+    raise NotImplementedError('{} does not support a tanh-Normal actor (TanhNormalProjection'
+                              'Network head); use it with SacAgent / SacPolicy.'.format(who))
+
+
 class ActorPolicy(tf_policy.TFPolicy):
 
   _SEED_TAG = _ACTOR_SEED_TAG
@@ -31,6 +38,7 @@ class ActorPolicy(tf_policy.TFPolicy):
 
   def __init__(self, time_step_spec, action_spec, actor_network, clip=True, collect=True, seed=0,
                info_spec=(), policy_state_spec=()):
+    reject_tanh_normal(actor_network, type(self).__name__)
     self._stateful_deterministic = False
     if getattr(actor_network, 'state_spec', ()) and not self._STATEFUL_ACTOR:
       if not getattr(actor_network, 'deterministic', False):

@@ -455,6 +455,43 @@ int b200rl_sac_alpha_loss(const float* logp, const float* weights, const float* 
  * (agents/ddpg/critic_network.py:163-178). */
 int b200rl_concat2(const float* a, int64_t lda, int64_t da, const float* b, int64_t ldb,
                    int64_t db, int64_t N, float* out, void* stream);
+/* Recurrent SAC: the three losses over the [B, T-1] transitions of [B, T] sequences
+ * (sac_agent.py with data_converter.AsTransition(squeeze_time_dim=False)).  Row r = b*(T-1) + t
+ * of q1, q2, tq1, tq2, next_logp, logp and of every per-row gradient is transition t of
+ * sequence b; log_alpha_dev is read on the device.
+ *   reward, discount  element (b, t) at ptr[b*ld + t*stride], read in place from the [B, T]
+ *                     experience (transition t reads step t)
+ *   weights           optional, weights[b*weight_stride] (0: one scalar, 1: one per row); a row of
+ *                     weight 0 adds exactly 0, even where its loss is inf or nan
+ * critic: y = reward_scale*r + gamma*d*(min(tq1,tq2) - exp(log_alpha)*next_logp);
+ *   loss = loss_weight * sum_b w_b sum_t ((y-q1)^2 + (y-q2)^2) / B (no LAST mask, as the
+ *   reference); dq_i = -2 (y - q_i) loss_weight w_b / B.
+ * actor: loss = loss_weight * sum_b w_b sum_t (exp(log_alpha)*logp - min(q1,q2)) / B; dlogp, and
+ *   dq1 / dq2 with the min's gradient on q1 where q1 <= q2.
+ * alpha: loss = loss_weight * coef * sum_b w_b sum_t (-logp - target_entropy) / B, coef =
+ *   log_alpha (use_log_alpha) or exp(log_alpha); dlog_alpha [1].
+ * partials: >= B200RL_SAC_SEQ_MAX_BLOCKS floats of scratch; ticket: a uint32 that is 0 before the
+ * launch and is left at 0.  Fixed-order sums: repeated calls return the same bits, and with
+ * T = 2 the per-row gradients equal the feed-forward kernels' bits.  nan_flag may be NULL. */
+#define B200RL_SAC_SEQ_MAX_BLOCKS 1024
+int b200rl_sac_seq_critic_loss(const float* q1, const float* q2, const float* tq1,
+                               const float* tq2, const float* next_logp, const float* reward,
+                               const float* discount, int64_t ld, int64_t stride,
+                               const float* weights, int64_t weight_stride,
+                               const float* log_alpha_dev, int64_t B, int64_t T, float gamma,
+                               float reward_scale, float loss_weight, float* loss, float* dq1,
+                               float* dq2, int32_t* nan_flag, float* partials, uint32_t* ticket,
+                               void* stream);
+int b200rl_sac_seq_actor_loss(const float* q1, const float* q2, const float* logp,
+                              const float* weights, int64_t weight_stride,
+                              const float* log_alpha_dev, int64_t B, int64_t T, float loss_weight,
+                              float* loss, float* dlogp, float* dq1, float* dq2, int32_t* nan_flag,
+                              float* partials, uint32_t* ticket, void* stream);
+int b200rl_sac_seq_alpha_loss(const float* logp, const float* weights, int64_t weight_stride,
+                              const float* log_alpha_dev, int64_t B, int64_t T,
+                              float target_entropy, int use_log_alpha, float loss_weight,
+                              float* loss, float* dlog_alpha, int32_t* nan_flag, float* partials,
+                              uint32_t* ticket, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * TD3 (agents/td3/td3_agent.py, agents/ddpg/actor_network.py)
