@@ -31,6 +31,7 @@ constexpr int kLstmMaxH = 256;
 constexpr int kLstmMaxThreads = 384;
 constexpr int64_t kLstmUBytes = 128 * 1024;     // resident U slice per CTA
 constexpr int64_t kLstmSmemMax = 227 * 1024;    // opt-in shared memory per block on sm_90
+constexpr int64_t kLstmMaxTiles = 65535;        // gridDim.y limit: tiles of BT rows per launch
 constexpr int kStepFirst = 0;
 
 __device__ __forceinline__ void cp_async4(float* dst, const float* src, bool valid) {
@@ -370,6 +371,11 @@ int b200rl_lstm_plan(int64_t B, int64_t H, int* cluster, int* rows_fwd, int* row
   int df = 0, db = 0;
   B200RL_CHECK_ARG(lstm_plan(B, (int)H, false, &gf, &df) && lstm_plan(B, (int)H, true, &gb, &db),
                    "lstm_plan: no tile fits shared memory");
+  const int bt = gf.BT < gb.BT ? gf.BT : gb.BT;
+  B200RL_CHECK_ARG((B + bt - 1) / bt <= kLstmMaxTiles,
+                   "lstm_plan: B = %lld needs more than %lld tiles of %d rows; B must be <= %lld "
+                   "for %lld units", (long long)B, (long long)kLstmMaxTiles, bt,
+                   (long long)(kLstmMaxTiles * bt), (long long)H);
   if (cluster) *cluster = gf.cs;
   if (rows_fwd) *rows_fwd = gf.BT;
   if (rows_bwd) *rows_bwd = gb.BT;
@@ -391,6 +397,10 @@ int b200rl_lstm_seq_fwd(const float* xw, const float* U, const int32_t* step_typ
   LstmTile g;
   int d = 0;
   B200RL_CHECK_ARG(lstm_plan(B, (int)H, false, &g, &d), "lstm_seq_fwd: no tile fits");
+  B200RL_CHECK_ARG((B + g.BT - 1) / g.BT <= kLstmMaxTiles,
+                   "lstm_seq_fwd: B = %lld needs more than %lld tiles of %d rows; B must be <= %lld "
+                   "for %lld units", (long long)B, (long long)kLstmMaxTiles, g.BT,
+                   (long long)(kLstmMaxTiles * g.BT), (long long)H);
   const size_t smem = (size_t)lstm_fwd_smem(g, d);
   const cudaStream_t st = (cudaStream_t)stream;
   if (d == 4)
@@ -412,6 +422,10 @@ int b200rl_lstm_seq_bwd(const float* dh, const float* gates, const float* c, con
   LstmTile g;
   int d = 0;
   B200RL_CHECK_ARG(lstm_plan(B, (int)H, true, &g, &d), "lstm_seq_bwd: no tile fits");
+  B200RL_CHECK_ARG((B + g.BT - 1) / g.BT <= kLstmMaxTiles,
+                   "lstm_seq_bwd: B = %lld needs more than %lld tiles of %d rows; B must be <= %lld "
+                   "for %lld units", (long long)B, (long long)kLstmMaxTiles, g.BT,
+                   (long long)(kLstmMaxTiles * g.BT), (long long)H);
   const size_t smem = (size_t)lstm_bwd_smem(g, d);
   const cudaStream_t st = (cudaStream_t)stream;
   if (d == 4)

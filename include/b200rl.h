@@ -760,7 +760,10 @@ int b200rl_act_bwd(const float* Y, const float* dY, float* dZ, int64_t n, int ac
  * (c0 is read for the forget-gate gradient of step 0).  U must be 16-byte aligned.
  * b200rl_lstm_plan: the launch shapes of the two kernels for (B, H): the cluster size (shared),
  * batch rows per cluster, cp.async ring depths and shared memory per CTA of each (the backward
- * takes fewer rows where its dG buffers leave no room for more; any output may be NULL). */
+ * takes fewer rows where its dG buffers leave no room for more; any output may be NULL).
+ * Each kernel runs ceil(B / rows) tiles along gridDim.y, so B may be at most 65535 * rows of that
+ * kernel (1 048 560 at 16 rows); a larger B is rejected with B200RL_ERR_INVALID before any launch,
+ * and b200rl_lstm_plan rejects a B past either kernel's limit. */
 int b200rl_lstm_plan(int64_t B, int64_t H, int* cluster, int* rows_fwd, int* rows_bwd,
                      int* depth_fwd, int* depth_bwd, int64_t* smem_fwd, int64_t* smem_bwd);
 int b200rl_lstm_seq_fwd(const float* xw, const float* U, const int32_t* step_type,
